@@ -41,6 +41,10 @@ def test_key(nodeid):
 
 
 def _next_key(key=None):
+    """The record of the next oracle env: `key` as given when it names one env ("<test key>#<n>", which is how
+    a test replays another test's record), else the test's key numbered by the envs it created so far."""
+    if key and "#" in key:
+        return key
     base = key or test_key(os.environ.get("PYTEST_CURRENT_TEST", "unkeyed"))
     k = _counters.get(base, 0)
     _counters[base] = k + 1
@@ -118,17 +122,37 @@ def oracle_env(num, env_name, lib_path, key=None, **kw):
     """The oracle on the stand-in pack while recording; else `lib_path` (the library under test) on it."""
     if recording_dir():
         kw.pop("extra_options", None)  # options of the library under test; the oracle takes its switches from the environment
+        kw.pop("launch_shape", None)   # how the library under test cuts a step into launches: not an input of the outputs
         env = RefVecEnv(num, env_name, lib_path=REF_LIB, pack_path=STANDIN_PACK, **kw)
     else:
         env = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=STANDIN_PACK, **kw)
     return Checked(env, _next_key(key))
 
 
-def merge(record_dir, out=RECORDS):
+def merge(record_dir, out=RECORDS, replace=False):
+    """Add the records of a recording run (PG_ORACLE_RECORD_DIR) to `out`, keeping every record already in it.
+    A key that is already there must come back with the same digests (re-recording an existing test is how
+    a recording machine shows it reproduces the oracle); replace=True lets the new digests win instead.
+    Returns (records in `out`, keys added, keys re-recorded identically)."""
     recs = {}
+    if os.path.exists(out):
+        with gzip.open(out, "rt") as f:
+            recs = json.load(f)
+    added, same, changed = [], [], []
     for fn in sorted(os.listdir(record_dir)):
         with open(os.path.join(record_dir, fn)) as f:
-            recs.update(json.load(f))
+            for key, marks in json.load(f).items():
+                if key not in recs:
+                    added.append(key)
+                elif recs[key] == marks:
+                    same.append(key)
+                else:
+                    changed.append(key)
+                    if not replace:
+                        continue
+                recs[key] = marks
+    if changed and not replace:
+        raise ValueError(f"{len(changed)} existing records would change (pass replace=True to overwrite): {changed[:8]}")
     with gzip.GzipFile(out, "wb", mtime=0) as f:
         f.write(json.dumps(recs, sort_keys=True, separators=(",", ":")).encode())
-    return len(recs)
+    return len(recs), added, same

@@ -79,7 +79,11 @@ class RefVecEnv:
                  num_threads=0, center_agent=True, use_backgrounds=True, use_monochrome_assets=False,
                  restrict_themes=False, use_generated_assets=False, paint_vel_info=False,
                  use_sequential_levels=False, debug_mode=0, lib_path=None, pack_path=None, resource_root=None,
-                 extra_options=None):
+                 extra_options=None, launch_shape=None, ob_layout=None):
+        """launch_shape=(chunks, serialize): a library that exports pgb200_set_launch_shape cuts every step,
+        the initial reset included, into `chunks` env chunks per game (launches back to back if serialize).
+        ob_layout: env e's observation goes to frame ob_layout[e] of a separate array (a non-contiguous
+        set of observation pointers, as a caller with its own buffer layout passes them)."""
         lib_path = lib_path or REF_LIB
         if not os.path.exists(lib_path):
             raise FileNotFoundError(f"{lib_path} missing — run python oracle/build_ref.py in the build container")
@@ -105,6 +109,7 @@ class RefVecEnv:
             L.set_state.restype = None
         self.num = num
         self._keep = []
+        self._ob_layout = None
         opts = dict(
             env_name=env_name, num_levels=num_levels, start_level=start_level, num_actions=15,
             use_sequential_levels=bool(use_sequential_levels), debug_mode=debug_mode, rand_seed=rand_seed,
@@ -116,6 +121,10 @@ class RefVecEnv:
             distribution_mode=DISTRIBUTION_MODE[distribution_mode])
         opts.update(extra_options or {})
         self.h = L.libenv_make(num, make_options(self._keep, **opts))
+        if launch_shape is not None and hasattr(L, "pgb200_set_launch_shape"):
+            L.pgb200_set_launch_shape.argtypes = [C.c_void_p, C.c_int, C.c_int]
+            L.pgb200_set_launch_shape.restype = None
+            L.pgb200_set_launch_shape(self.h, int(launch_shape[0]), int(bool(launch_shape[1])))
         n_info = L.libenv_get_tensortypes(self.h, SPACE_INFO, None)
         info_types = (TensorType * n_info)()
         L.libenv_get_tensortypes(self.h, SPACE_INFO, info_types)
@@ -132,7 +141,14 @@ class RefVecEnv:
             self.info[t.name.decode()] = arr
             for e in range(num):
                 info_ptrs[si * num + e] = arr.ctypes.data + e * arr.itemsize
-        ob_ptrs = (C.c_void_p * num)(*[self.rgb.ctypes.data + e * 64 * 64 * 3 for e in range(num)])
+        if ob_layout is None:
+            ob_ptrs = (C.c_void_p * num)(*[self.rgb.ctypes.data + e * 64 * 64 * 3 for e in range(num)])
+        else:
+            # the caller's observation slots are not one contiguous [num][64][64][3] block: env e writes
+            # frame ob_layout[e] of a larger array, and self.rgb is the env-ordered view of it
+            self._ob_store = np.zeros((int(max(ob_layout)) + 1, 64, 64, 3), np.uint8)
+            ob_ptrs = (C.c_void_p * num)(*[self._ob_store.ctypes.data + int(s) * 64 * 64 * 3 for s in ob_layout])
+            self._ob_layout = np.asarray(ob_layout)
         ac_ptrs = (C.c_void_p * num)(*[self.ac.ctypes.data + e * 4 for e in range(num)])
         self._bufs = Buffers(ob_ptrs, self.rew.ctypes.data_as(C.POINTER(C.c_float)),
                              self.first.ctypes.data_as(C.POINTER(C.c_uint8)), info_ptrs, ac_ptrs)
@@ -141,6 +157,8 @@ class RefVecEnv:
 
     def observe(self):
         self.lib.libenv_observe(self.h)
+        if self._ob_layout is not None:
+            self.rgb[:] = self._ob_store[self._ob_layout]
         return self.rew, {"rgb": self.rgb}, self.first
 
     def act(self, ac):

@@ -7,16 +7,21 @@ from oracle.record import STANDIN_PACK, oracle_env
 from oracle.ref_env import RefVecEnv, default_pack, mt19937_actions
 
 
-def make_pair(lib_path, num, env_name, extra_options=None, **kw):
+def make_pair(lib_path, num, env_name, extra_options=None, launch_shape=None, ob_layout=None, **kw):
+    """(the oracle, the library under test); launch_shape and ob_layout apply to the library under test only."""
     ref = RefVecEnv(num, env_name, **kw)
-    dut = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=default_pack(), extra_options=extra_options, **kw)
+    dut = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=default_pack(), extra_options=extra_options,
+                    launch_shape=launch_shape, ob_layout=ob_layout, **kw)
     return ref, dut
 
 
-def make_checked_pair(lib_path, num, env_name, extra_options=None, **kw):
-    """(oracle_env: the oracle's recorded outputs, the library under test), both on the stand-in asset pack."""
-    ref = oracle_env(num, env_name, lib_path, extra_options=extra_options, **kw)
-    dut = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=STANDIN_PACK, extra_options=extra_options, **kw)
+def make_checked_pair(lib_path, num, env_name, extra_options=None, launch_shape=None, ob_layout=None, key=None, **kw):
+    """(oracle_env: the oracle's recorded outputs, the library under test), both on the stand-in asset pack.
+    launch_shape and ob_layout apply to the library under test only; they are not inputs of the outputs, so a
+    run that only changes them may replay the record of another test (key)."""
+    ref = oracle_env(num, env_name, lib_path, key=key, extra_options=extra_options, **kw)
+    dut = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=STANDIN_PACK, extra_options=extra_options,
+                    launch_shape=launch_shape, ob_layout=ob_layout, **kw)
     return ref, dut
 
 

@@ -170,3 +170,86 @@ def test_whole_world_view_of_scrolling_games(ref_lib, hostsim_lib, name, mode):
     run_lockstep(ref, dut, 200)
     ref.close()
     dut.close()
+
+
+# ---- launch shapes: VecEnv::launch cuts a step into (game, env chunk) launches; at benchmark sizes a
+# step has 8 chunks per game. pgb200_set_launch_shape forces the chunk count here, so the chunk index
+# arithmetic (env_first = g + lo * G, env_step = G, uneven and empty chunks) runs at oracle sizes.
+@pytest.mark.parametrize("name,n,chunks", [
+    ("coinrun", 16, 3),        # uneven chunks (5, 5, 6)
+    ("coinrun", 16, 16),       # one env per chunk
+    ("coinrun", 16, 40),       # 24 empty chunks
+    ("coinrun", 13, 4),        # odd n: partial setup / logic blocks in every chunk
+    (ALL_GAMES, 32, 5),        # joint list: 2 envs per game in 5 chunks, 3 of them empty
+    (ALL_GAMES, 64, 3),        # joint list: 4 envs per game in 3 uneven chunks
+    ("caveflyer,heist,starpilot", 21, 3),
+])
+def test_forced_launch_shapes_bit_exact(ref_lib, hostsim_lib, name, n, chunks):
+    ref, dut = make_pair(hostsim_lib, n, name, launch_shape=(chunks, False), distribution_mode="hard", num_levels=200,
+                         start_level=0, rand_seed=0)
+    run_lockstep(ref, dut, 200)
+    ref.close()
+    dut.close()
+
+
+@pytest.mark.parametrize("name,n", [("coinrun", 1), ("coinrun", 3), ("coinrun", 13), ("heist", 5), ("bossfight", 7),
+                                    ("caveflyer,heist,starpilot", 21)])
+def test_odd_env_counts_bit_exact(ref_lib, hostsim_lib, name, n):
+    """Env counts that leave a partial block in every kernel (4 envs per setup block, 2 per logic block)."""
+    ref, dut = make_pair(hostsim_lib, n, name, distribution_mode="hard", num_levels=200, start_level=0, rand_seed=0)
+    run_lockstep(ref, dut, 300)
+    ref.close()
+    dut.close()
+
+
+@pytest.mark.parametrize("name,n,chunks", [(ALL_GAMES, 16, 3), ("caveflyer,heist,starpilot", 9, 2)])
+def test_state_blobs_into_joint_list(ref_lib, hostsim_lib, name, n, chunks):
+    """set_state into a joint list: env e is game e % G (gi = env_idx % G), re-rendered by a one-env launch;
+    the fresh envs the blobs are loaded into step in forced chunks afterwards."""
+    from oracle.ref_env import RefVecEnv, default_pack
+
+    kw = dict(distribution_mode="hard", num_levels=200, start_level=0)
+    run_state_roundtrip(lambda seed: RefVecEnv(n, name, rand_seed=seed, **kw),
+                        lambda seed: RefVecEnv(n, name, rand_seed=seed, lib_path=hostsim_lib, resource_root=default_pack(),
+                                               launch_shape=(chunks, False), **kw),
+                        n, 100)
+
+
+def test_set_state_leaves_other_envs_alone(ref_lib, hostsim_lib):
+    """Loading one env of a chunk changes that env only: the others go on exactly as in a run without it."""
+    import numpy as np
+
+    from oracle.ref_env import RefVecEnv, default_pack, mt19937_actions
+
+    kw = dict(distribution_mode="hard", num_levels=200, start_level=0, rand_seed=0, lib_path=hostsim_lib,
+              resource_root=default_pack(), launch_shape=(3, False))
+    n, names = 24, "caveflyer,heist,starpilot"
+    a, b = RefVecEnv(n, names, **kw), RefVecEnv(n, names, **kw)
+    donor = RefVecEnv(n, names, **dict(kw, rand_seed=9))
+    acts = mt19937_actions(4, n, 120)
+    for t in range(60):
+        for env in (a, b, donor):
+            env.act(acts[t])
+    targets = [1, 11, 22]
+    for e in targets:
+        b.set_state(e, donor.get_state(e))
+    others = np.setdiff1d(np.arange(n), targets)
+    for t in range(60, 120):
+        for env in (a, b, donor):
+            env.act(acts[t])
+            env.observe()
+        assert np.array_equal(a.rgb[others], b.rgb[others]) and np.array_equal(a.rew[others], b.rew[others]), f"step {t}"
+        assert np.array_equal(donor.rgb[targets], b.rgb[targets]) and np.array_equal(donor.first[targets], b.first[targets]), f"step {t}"
+    for env in (a, b, donor):
+        env.close()
+
+
+def test_staging_path_with_scattered_observation_slots(ref_lib, hostsim_lib):
+    """Observation pointers that are not one contiguous block (reversed env order, every other frame of a
+    larger array) take the staging buffer and the per-env scatter."""
+    layout = [2 * (12 - 1 - e) for e in range(12)]
+    ref, dut = make_pair(hostsim_lib, 12, "maze", launch_shape=(5, False), ob_layout=layout, distribution_mode="hard",
+                         num_levels=200, start_level=0, rand_seed=0)
+    run_lockstep(ref, dut, 200)
+    ref.close()
+    dut.close()

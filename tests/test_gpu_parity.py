@@ -239,6 +239,7 @@ def test_state_blobs_remaining_games(product_lib, name):
     ("maze", "hard", 32768, 30, 200),      # configs[3]
     ("bigfish", "hard", 65536, 30, 150),   # configs[2]
     (ALL16, "hard", 32768, 30, 150),       # configs[4], one GPU's share
+    ("bigfish,coinrun", "hard", 65536, 30, 150),  # a joint list in 8 chunks per game: env_first = g + lo * G
 ])
 def test_mid_array_envs_match_oracle(product_lib, name, mode, n_big, warm, steps):
     """Benchmark-size run, envs picked from EVERY launch chunk (not just the first 64): their state is
