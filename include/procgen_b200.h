@@ -156,6 +156,21 @@ struct pgb200_device_buffers {
  * libenv_set_buffers does in host mode). Pointers stay valid until libenv_close. */
 LIBENV_API int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *out);
 
+/* Per-env level choice: `*out` = this handle's int32 array next_level_seed[num_envs] (device memory;
+ * host memory in the CPU debug build), allocated and filled with -1 by the first call, which also
+ * performs the initial reset if it has not happened yet. The pointer stays valid until libenv_close.
+ * At every reset inside a step (an episode end, the timeout, or action -1), env e reads
+ * s = next_level_seed[e]: s >= 0 makes the new level's seed s instead of a draw from the env's
+ * level_seed_rand_gen (not advanced) or the +997 of use_sequential_levels (later levels continue from
+ * s + 997), and the step writes -1 back (the override is consumed); s < 0 leaves the reset as it is. Any
+ * s in [0, 2^31) is accepted, also outside [start_level, start_level + num_levels). Indices are the
+ * handle's own (env n of a joint list plays game n % G; local indices of a shard). The initial reset
+ * is not affected; to start envs on chosen levels, write overrides and step once with action -1.
+ * get_state / set_state neither read nor write the array (pending overrides survive set_state).
+ * Ordering: with pgb200_act_device, write the array on the handle's stream before the call, like the
+ * action buffer; with libenv_act, the writes must be complete before the call. Returns 0. */
+LIBENV_API int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is

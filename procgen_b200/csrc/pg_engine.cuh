@@ -787,11 +787,17 @@ struct Engine {
     }
 
     // ---- Game::reset / Game::step (game.cpp:93-155)
-    static PG_HD void reset(Ctx &c) {
+    // level_seed_override >= 0 (pgb200_get_next_level_seeds) replaces the draw of the next level seed and
+    // nothing else: level_seed_rand_gen is not advanced. Returns whether the override was taken.
+    static PG_HD bool reset(Ctx &c, int32_t level_seed_override = -1) {
         EnvHdr &h = *c.h;
+        bool took = false;
         h.reset_count++;
         if (h.episodes_remaining == 0) {
-            if (h.options.use_sequential_levels && h.level_complete) {
+            if (level_seed_override >= 0) {
+                h.current_level_seed = level_seed_override;
+                took = true;
+            } else if (h.options.use_sequential_levels && h.level_complete) {
                 h.current_level_seed = (int32_t)((uint32_t)h.current_level_seed + 997u);
             } else {
                 h.current_level_seed = rand_randint(*c.lvl_rng, h.level_seed_low, h.level_seed_high);
@@ -808,11 +814,13 @@ struct Engine {
         h.total_reward = 0;
         h.episodes_remaining -= 1;
         h.action = h.default_action;
+        return took;
     }
 
     // Game::step (game.cpp:120-155) in two halves, so that the vector runtime can run level generation
     // (the reset of an episode that just ended) as a separate pass: step_play = everything up to the
-    // decision `if (step_data.done) reset()`, returns that decision; step_finish = the rest.
+    // decision `if (step_data.done) reset()`, returns that decision; step_finish = the rest, returns whether
+    // its reset took level_seed_override.
     static PG_HD bool step_play(Ctx &c) {
         EnvHdr &h = *c.h;
         h.cur_time += 1;
@@ -834,15 +842,17 @@ struct Engine {
         h.prev_level_seed = h.current_level_seed;
         return h.done != 0;
     }
-    static PG_HD void step_finish(Ctx &c, bool do_reset) {
+    static PG_HD bool step_finish(Ctx &c, bool do_reset, int32_t level_seed_override) {
         EnvHdr &h = *c.h;
+        bool took = false;
         if (do_reset)
-            reset(c);
+            took = reset(c, level_seed_override);
         if (h.options.use_sequential_levels && h.level_complete)
             h.done = 0;
         h.episode_done = h.done;
+        return took;
     }
-    static PG_HD void step(Ctx &c) { step_finish(c, step_play(c)); }
+    static PG_HD void step(Ctx &c) { step_finish(c, step_play(c), -1); }
 };
 
 // ---------------------------------------------------------------- default hooks (the virtuals)

@@ -30,6 +30,7 @@ struct KParams {
     uint8_t *info_prev_level_complete;
     int32_t *info_level_seed;
     const uint32_t *lvl_seeds;  // per-env seed for level_seed_rand_gen (vecgame.cpp:301-314)
+    int32_t *next_level_seed;   // optional [N] caller-chosen seed of the env's next level, -1 = none; null = off
     // strides (elements)
     int32_t ent_stride;         // ent_cap + 1 (ghost slot)
     int32_t grid_stride;
@@ -146,14 +147,25 @@ __device__ __forceinline__ void env_prefetch(const KParams &p, int env) {
 #endif
 
 // Game::step (game.cpp:120-155) up to, not including, the pixel work. One thread.
-template <class G, class Frame>
+// LEVEL_CHOICE: the handle has a next_level_seed array. A separate instantiation, so that the logic kernel
+// of a handle without one carries no trace of the feature (not even registers held across the step).
+template <class G, class Frame, bool LEVEL_CHOICE = false>
 PG_HD void env_step_logic(const KParams &p, int env) {
 #if defined(__CUDA_ARCH__)
     env_prefetch(p, env);
 #endif
     Ctx c = make_ctx(p, env);
     c.h->action = p.action[env];  // vecgame.cpp:388
-    Engine<G>::step(c);
+    if (LEVEL_CHOICE) {
+        const bool do_reset = Engine<G>::step_play(c);
+        // the caller's choice of the next level is read only by a step that resets, and consumed when that
+        // reset takes it
+        const int32_t next_seed = do_reset ? p.next_level_seed[env] : -1;
+        if (Engine<G>::step_finish(c, do_reset, next_seed))
+            p.next_level_seed[env] = -1;
+    } else {
+        Engine<G>::step(c);
+    }
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, *c.h);
 }

@@ -69,7 +69,7 @@ constexpr int kRenderThreads = 128;
 // Persistent: the grid is sized to fill the machine once and every warp pulls env indices from a
 // global ticket counter until the launch's range is exhausted, so a long env (level reset) only
 // delays its own warp and no SM slot idles waiting for a block launch.
-template <class G, bool INIT>
+template <class G, bool INIT, bool LEVEL_CHOICE = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
         if (INIT)
             env_init_logic<G, Frame>(p, env);
         else
-            env_step_logic<G, Frame>(p, env);
+            env_step_logic<G, Frame, LEVEL_CHOICE>(p, env);
         __syncwarp();
         if (p.dbg_cycles && lane == 0)
             p.dbg_cycles[env] = (uint32_t)(clock64() - t0);
@@ -355,7 +355,10 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, sizeof(unsigned int), ls));
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[0], ls));
-    logic_kernel<G, INIT><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
+    if (!INIT && p.next_level_seed)
+        logic_kernel<G, false, true><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
+    else
+        logic_kernel<G, INIT><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
     if (lc.logic_stream) {
         CUDA_CHECK(cudaEventRecord(lc.link, ls));
         CUDA_CHECK(cudaStreamWaitEvent(lc.stream, lc.link, 0));
@@ -376,6 +379,8 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
         int env = p.env_first + b * p.env_step;
         if (INIT)
             env_init_logic<G, Frame>(p, env);
+        else if (p.next_level_seed)
+            env_step_logic<G, Frame, true>(p, env);
         else
             env_step_logic<G, Frame>(p, env);
         render_env_serial<G, VIEW, Frame>(p, env, *f);

@@ -223,6 +223,7 @@ struct VecEnv {
     SpriteDesc *d_tile_sprites = nullptr;
     uint32_t *d_lvl_seeds = nullptr;
     int32_t *d_action = nullptr;
+    int32_t *d_next_level_seed = nullptr;   // allocated by the first pgb200_get_next_level_seeds
     bool initial_reset_done = false;
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
@@ -930,6 +931,7 @@ void libenv_close(libenv_env *handle) {
     dev_free(v->d_tile_index);
     dev_free(v->d_tile_sprites);
     dev_free(v->d_action);
+    dev_free(v->d_next_level_seed);
     dev_free(p.rgb);
     dev_free(p.rew);
     dev_free(p.first);
@@ -998,6 +1000,27 @@ int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *
 #else
     out->stream = nullptr;
 #endif
+    return 0;
+}
+
+int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    v->ensure_initial_reset();
+    if (!v->d_next_level_seed) {
+        const size_t N = (size_t)v->num_envs;
+#ifndef PG_HOSTSIM
+        CUDA_CHECK(cudaMalloc((void **)&v->d_next_level_seed, (N ? N : 1) * sizeof(int32_t)));
+        CUDA_CHECK(cudaMemsetAsync(v->d_next_level_seed, 0xff, N * sizeof(int32_t), v->stream));  // every entry -1
+        // complete before the caller writes, from whatever stream it writes on
+        v->sync();
+#else
+        v->d_next_level_seed = (int32_t *)malloc((N ? N : 1) * sizeof(int32_t));
+        for (size_t e = 0; e < N; e++) v->d_next_level_seed[e] = -1;
+#endif
+        v->base.next_level_seed = v->d_next_level_seed;
+    }
+    *out = v->d_next_level_seed;
     return 0;
 }
 

@@ -135,6 +135,7 @@ class BaseProcgenEnv:
         })
         self._host_buffers = bool(host_buffers)
         self._torch = None
+        self._next_level_seeds = None
         if self._lib.pgb200_is_device_build():
             import torch
 
@@ -241,6 +242,10 @@ class BaseProcgenEnv:
         """env.py:197-200: actions are cast to int32. Asynchronous, like VecGame::act."""
         if self._host_buffers:
             self._ac[:] = np.asarray(ac).astype(np.int32)
+            if self._next_level_seeds is not None:
+                # libenv_act reads the level choices on the library's own stream: the caller's torch writes
+                # must be complete first
+                self._torch.cuda.current_stream(self._next_level_seeds.device).synchronize()
             self._lib.libenv_act(self._h)
             return
         torch = self._torch
@@ -286,6 +291,28 @@ class BaseProcgenEnv:
     def get_info_tensors(self):
         """Column form of get_info() without a host copy."""
         return dict(self._info)
+
+    def next_level_seeds(self):
+        """int32 CUDA tensor [num] aliasing the library's per-env choice of the next level (allocated, all -1,
+        on the first call). At every reset inside a step (episode end, timeout, or action -1) env e checks its
+        entry s: s >= 0 starts the new level with seed s — any seed in [0, 2**31), also outside
+        [start_level, start_level + num_levels) — and the step sets the entry back to -1 (an override is used
+        once); s = -1 leaves the reset as it is (a draw from the env's own level seed generator, which an
+        override does not advance, or the +997 of use_sequential_levels). The initial reset is not affected:
+        to start envs on chosen levels, write seeds and act() with action -1 for them. get_state / set_state
+        neither read nor change the array.
+
+        Write it with torch ops on the stream you step on (device-resident mode); with host_buffers=True,
+        act() waits for the current torch stream before it starts the step."""
+        if self._next_level_seeds is None:
+            torch = self._torch
+            ptr = C.POINTER(C.c_int32)()
+            with torch.cuda.device(self.device_index):
+                if self._lib.pgb200_get_next_level_seeds(self._h, C.byref(ptr)) != 0:
+                    raise RuntimeError("pgb200_get_next_level_seeds failed")
+                dev = torch.device("cuda", self.device_index)
+                self._next_level_seeds = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "<i4"), device=dev)
+        return self._next_level_seeds
 
     def callmethod(self, method: str, *args, **kwargs):
         return getattr(self, method)(*args, **kwargs)
@@ -451,6 +478,7 @@ class BaseProcgenEnv:
             self._lib.pgb200_set_rgb_mirror(self._h, None, None)
             self._peer = None
         if getattr(self, "_h", None):
+            self._next_level_seeds = None
             self._lib.libenv_close(self._h)
             self._h = None
 

@@ -49,7 +49,7 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_sync", "pgb200_get_errors", "pgb200_debug_cycles", "pgb200_debug_read_env", "pgb200_kernel_launches", "pgb200_is_device_build",
            "pgb200_kernel_timing_begin", "pgb200_kernel_timing_end", "get_state", "set_state", "pgb200_set_launch_shape",
            "pgb200_frame_info", "pgb200_set_rgb_mirror", "pgb200_mirror_parity",
-           "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset"]
+           "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds"]
 
 _lib = None
 
@@ -67,6 +67,8 @@ def bind(lib):
         f.restype = None
     lib.pgb200_get_device_buffers.argtypes = [C.c_void_p, C.POINTER(DeviceBuffers)]
     lib.pgb200_get_device_buffers.restype = C.c_int
+    lib.pgb200_get_next_level_seeds.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
+    lib.pgb200_get_next_level_seeds.restype = C.c_int
     lib.pgb200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     lib.pgb200_set_stream.restype = None
     lib.pgb200_get_errors.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
