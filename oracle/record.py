@@ -59,6 +59,20 @@ def _load():
     return _records
 
 
+def use_records(path):
+    """Make the records of another record file (e.g. tests/golden/level_seed_records.json.gz) replayable through
+    oracle_env beside those of RECORDS. A file of its own keeps a new test file's records apart from the
+    existing ones; its keys are its tests' own, and a key in both files must hold the same digests."""
+    if recording_dir():
+        return
+    recs = _load()
+    with gzip.open(path, "rt") as f:
+        extra = json.load(f)
+    clash = [k for k in extra if k in recs and recs[k] != extra[k]]
+    assert not clash, f"records in {os.path.basename(path)} and {os.path.basename(RECORDS)} differ: {clash[:4]}"
+    recs.update(extra)
+
+
 class Checked:
     """An env of the libenv ABI (RefVecEnv) whose outputs are checked against, or recorded as, the oracle's."""
 

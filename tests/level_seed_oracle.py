@@ -7,8 +7,6 @@ implementation of the libenv ABI (the oracle itself, or the oracle's records rep
 under test), so a run with overrides can be compared with the reference bit for bit.
 """
 import ctypes as C
-import gzip
-import json
 import os
 import struct
 
@@ -23,18 +21,10 @@ LEVEL_SEED_RECORDS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "g
 
 
 def use_level_seed_records():
-    """Make the records of LEVEL_SEED_RECORDS replayable through oracle.record.oracle_env. Their keys are the new
-    tests' own, so none of them can stand for a record of the main file."""
-    from oracle import record
+    """Make the records of LEVEL_SEED_RECORDS replayable through oracle.record.oracle_env."""
+    from oracle.record import use_records
 
-    if record.recording_dir():
-        return
-    recs = record._load()
-    with gzip.open(LEVEL_SEED_RECORDS, "rt") as f:
-        extra = json.load(f)
-    clash = [k for k in extra if k in recs and recs[k] != extra[k]]
-    assert not clash, f"records in both files differ: {clash[:4]}"
-    recs.update(extra)
+    use_records(LEVEL_SEED_RECORDS)
 
 # the fixed-size scalar header of the blob, in wire order (oracle/state_blob.py parse)
 _OPTION_INTS = ["paint_vel_info", "use_generated_assets", "use_monochrome_assets", "restrict_themes", "use_backgrounds",
