@@ -180,7 +180,26 @@ LIBENV_API int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out);
 LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
 
 /* Steps every env with the actions currently in the device action buffer. Asynchronous: enqueues
- * on the handle's stream and returns. */
+ * on the handle's stream and returns.
+ *
+ * CUDA graph capture. pgb200_act_device may be called while the handle's stream captures a CUDA graph
+ * (cudaStreamBeginCapture, or pgb200_set_stream onto a stream that is capturing: that rebinding does not
+ * wait). Every launch of the step, its ticket memsets and the fork to / join from the handle's auxiliary
+ * streams become nodes of the caller's graph, and the consumer ring position advances on the device, so a
+ * replay is the step issued at capture: same outputs as an eager call on the same inputs.
+ * A captured step keeps what the host decided at capture: the launch shape (pgb200_set_launch_shape), the
+ * level choice (the next_level_seed array is read only if pgb200_get_next_level_seeds had been called
+ * before the capture), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
+ * any of these afterwards leaves the graph as it was; capture again. Replays of one handle's graphs must be
+ * ordered with each other and with its eager work (one stream, or events). pgb200_kernel_launches counts
+ * launches issued, a captured step once, not its replays.
+ * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
+ * pgb200_get_errors, or a fatal message where the call returns nothing): the first
+ * pgb200_get_next_level_seeds, pgb200_get_device_buffers before the initial reset, pgb200_set_consumer_output,
+ * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
+ * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step
+ * cannot be captured with the peer mirror set (its parity is host state), with host buffers, or under
+ * kernel timing: pgb200_act_device then ends the process with a message. */
 LIBENV_API void pgb200_act_device(libenv_env *handle);
 
 /* Blocks until all enqueued work of this handle is complete (VecGame::wait_for_stepping_threads). */
@@ -217,9 +236,18 @@ LIBENV_API int pgb200_mirror_parity(libenv_env *handle);
  * (oldest first) is always the contiguous slot range [s + 1, s + k] (pgb200_consumer_slot = s). When
  * an env starts an episode the older frames of its window are zeroed (baselines' VecFrameStack). At
  * the call the current frames are written as step 0. buffer == NULL or dtype == 0 switches it off.
- * Returns 0, -1 on bad arguments or in the host debug build. */
+ * Returns 0, -1 on bad arguments or in the host debug build.
+ * The ring position lives on the device (pgb200_get_consumer_slot_device) and every step advances it
+ * there, ahead of its render kernels. pgb200_consumer_slot is the host's count of the steps issued since
+ * the call, mod k: the device value as long as every step is issued by pgb200_act_device / libenv_act,
+ * not by replaying a CUDA graph. */
 LIBENV_API int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int k_frames);
 LIBENV_API int pgb200_consumer_slot(libenv_env *handle);
+/* `*out` = this handle's device-resident int32 ring position s of the consumer output (the slot the
+ * latest step wrote), for a captured consumer that indexes the ring without the host: the ordered stack
+ * is slots [s + 1, s + k]. Written on the handle's stream. Valid until libenv_close. Returns 0, or -1
+ * in the host debug build. */
+LIBENV_API int pgb200_get_consumer_slot_device(libenv_env *handle, int32_t **out);
 
 /* Profiling variant only (-DPG_PHASE_TIMING): byte offset of the 12 phase-cycle counters inside the
  * header pgb200_debug_read_env returns; -1 in the product build. */
@@ -229,7 +257,8 @@ LIBENV_API int pgb200_debug_phase_offset(void);
  * per SM the render kernel of `game` is compiled for. Returns -1 for an unknown game. */
 LIBENV_API int pgb200_frame_info(const char *game, int *frame_bytes, int *ctas_per_sm);
 
-/* Number of CUDA kernels this handle has launched so far (bench accounting). */
+/* Number of CUDA kernels this handle has launched so far (bench accounting): launches issued, so a step
+ * captured in a CUDA graph counts once and its replays do not. */
 LIBENV_API int64_t pgb200_kernel_launches(libenv_env *handle);
 
 /* Per-kernel device timing for measurement (bench.py roofline): between begin and end every

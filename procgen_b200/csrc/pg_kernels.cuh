@@ -53,7 +53,7 @@ struct KParams {
     void *consumer;             // [N][slots][3][64][64] 16-bit elements; null = off
     const uint16_t *consumer_lut;  // [256] = (16-bit float)(v / 255.f)
     int32_t consumer_k;         // frames per stack; slots = k == 1 ? 1 : 2k
-    int32_t consumer_slot;      // ring position this step writes: t mod k
+    const int32_t *consumer_slot_dev;  // device: ring position this step writes, t mod k (advanced on the device once per step)
     uint32_t *dbg_cycles;       // optional [N] per-env logic duration in SM cycles (profiling aid)
 };
 

@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
         // Consumer epilogue: the frame as normalised 16-bit floats, planar, into ring slot s (and its
         // twin s + k); an env that starts an episode this step gets the older frames of its window
         // zeroed (the frame-stack convention of baselines' VecFrameStack). Thread = pixel pairs.
-        const int kf = p.consumer_k, s = p.consumer_slot;
+        const int kf = p.consumer_k, s = *p.consumer_slot_dev;
         const int slots = kf == 1 ? 1 : 2 * kf;
         uint32_t *base = reinterpret_cast<uint32_t *>(p.consumer) + (size_t)env * slots * (3 * RES_W * RES_H / 2);
         const uint16_t *lut = p.consumer_lut;

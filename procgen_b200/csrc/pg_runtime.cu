@@ -205,6 +205,23 @@ __global__ void consumer_lut_kernel(uint16_t *lut, int bf16) {
         lut[v] = __half_as_ushort(__float2half_rn(x));
     }
 }
+
+// The consumer ring position of the coming step, advanced on the device so that a step captured in a CUDA
+// graph moves it on at every replay (a kernel argument would be frozen at capture)
+__global__ void consumer_advance_kernel(int32_t *slot, int k) { *slot = (*slot + 1) % k; }
+
+// Whether `s` is capturing a CUDA graph. Querying the legacy stream while another stream captures in a
+// non-relaxed mode reports cudaErrorStreamCaptureImplicit: work there would join that capture, so it counts.
+static bool stream_capturing(cudaStream_t s) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(s, &st);
+    if (e == cudaErrorStreamCaptureImplicit) {
+        cudaGetLastError();
+        return true;
+    }
+    CUDA_CHECK(e);
+    return st != cudaStreamCaptureStatusNone;
+}
 #endif
 
 // ================================================================= VecEnv (VecGame, vecgame.h)
@@ -259,7 +276,9 @@ struct VecEnv {
     uint8_t *mirror[2] = {nullptr, nullptr};
     int mirror_parity = 0;
     uint16_t *d_consumer_lut = nullptr;
-    int64_t consumer_steps = 0;
+    int32_t *d_consumer_slot = nullptr;  // the ring position the render kernels write (base.consumer_slot_dev)
+    int64_t consumer_steps = 0;          // host count of the steps issued since the consumer output was set
+    int32_t consumer_slot = 0;           // consumer_steps mod k: the device slot while every step is issued eagerly
     bool have_host_bufs = false;
     bool rgb_copy_enqueued = false;  // this step's observation DMA already follows the render kernels
     bool ob_direct = false;      // caller's obs block is contiguous and page-locked: DMA straight into it
@@ -303,6 +322,13 @@ struct VecEnv {
         if (force_chunks <= 0 && per_game < 4096 * chunks)
             chunks = 1;
 #ifndef PG_HOSTSIM
+        // the consumer ring moves on once per step, behind the previous step and ahead of every render
+        // kernel of this one (they all start after the fork below)
+        if (!init && base.consumer) {
+            consumer_advance_kernel<<<1, 1, 0, stream>>>(d_consumer_slot, base.consumer_k);
+            CUDA_CHECK(cudaGetLastError());
+            launches++;
+        }
         // more than one (logic, render) pair in the step — env chunks of one game, or the games of a
         // joint list — are spread over the auxiliary streams so they overlap on the SMs
         const int nstreams = (chunks * G > 1 && !serialize_launches) ? kAuxStreams : 0;
@@ -319,7 +345,7 @@ struct VecEnv {
             mirror_parity ^= 1;
         if (!init && base.consumer) {
             consumer_steps++;
-            base.consumer_slot = (int32_t)(consumer_steps % base.consumer_k);
+            consumer_slot = (int32_t)(consumer_steps % base.consumer_k);
         }
         int k = 0;
         for (int g = 0; g < G; g++) {
@@ -401,6 +427,21 @@ struct VecEnv {
 #ifndef PG_HOSTSIM
         CUDA_CHECK(cudaStreamSynchronize(stream));
 #endif
+    }
+
+    // True while the handle's stream captures a CUDA graph. The entry points that wait for the device or
+    // allocate then refuse (-1, or a fatal message where the call returns nothing): either would
+    // invalidate the caller's capture.
+    bool capturing() {
+#ifndef PG_HOSTSIM
+        return stream_capturing(stream);
+#else
+        return false;
+#endif
+    }
+    void refuse_in_capture(const char *what) {
+        if (capturing())
+            pg_fatal("%s cannot run while the handle's stream is capturing a CUDA graph\n", what);
     }
 
     void set_device() {
@@ -609,6 +650,8 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
             v->render_smem_floor &= ~15;
         }
         CUDA_CHECK(cudaMalloc((void **)&v->d_tickets, VecEnv::kMaxTickets * sizeof(unsigned int)));
+        v->d_consumer_slot = dev_alloc<int32_t>(1);
+        v->base.consumer_slot_dev = v->d_consumer_slot;
     }
     // sub_step <-> push_obj recurse to depth 5 on the logic thread
     {
@@ -840,6 +883,7 @@ static void fetch_to_host(VecEnv *v) {
 void libenv_set_buffers(libenv_env *handle, struct libenv_buffers *bufs) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    v->refuse_in_capture("libenv_set_buffers");
     const size_t N = (size_t)v->num_envs;
     pg_fassert(!v->initial_reset_done);
     v->h_ob.assign(bufs->ob, bufs->ob + N);  // one observation space
@@ -889,6 +933,7 @@ void libenv_set_buffers(libenv_env *handle, struct libenv_buffers *bufs) {
 void libenv_observe(libenv_env *handle) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    v->refuse_in_capture("libenv_observe");
     pg_fassert(v->have_host_bufs);
     fetch_to_host(v);
 }
@@ -896,6 +941,7 @@ void libenv_observe(libenv_env *handle) {
 void libenv_act(libenv_env *handle) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    v->refuse_in_capture("libenv_act");
     pg_fassert(v->have_host_bufs);
     const size_t N = (size_t)v->num_envs;
     v->sync();  // staging buffer reuse (wait_for_stepping_threads, vecgame.cpp:379)
@@ -913,6 +959,7 @@ void libenv_close(libenv_env *handle) {
     if (!v)
         return;
     v->set_device();
+    v->refuse_in_capture("libenv_close");
     v->sync();
     KParams &p = v->base;
     dev_free(p.hdr);
@@ -940,6 +987,7 @@ void libenv_close(libenv_env *handle) {
     dev_free(p.info_level_seed);
     dev_free(v->d_lvl_seeds);
     dev_free(v->d_consumer_lut);
+    dev_free(v->d_consumer_slot);
     if (p.dbg_cycles)
         dev_free(p.dbg_cycles);
 #ifndef PG_HOSTSIM
@@ -984,6 +1032,8 @@ void libenv_close(libenv_env *handle) {
 int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (!v->initial_reset_done && v->capturing())
+        return -1;
     v->ensure_initial_reset();
     const KParams &p = v->base;
     out->rgb = p.rgb;
@@ -1006,6 +1056,8 @@ int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *
 int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if ((!v->initial_reset_done || !v->d_next_level_seed) && v->capturing())
+        return -1;
     v->ensure_initial_reset();
     if (!v->d_next_level_seed) {
         const size_t N = (size_t)v->num_envs;
@@ -1027,10 +1079,15 @@ int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out) {
 void pgb200_set_stream(libenv_env *handle, void *stream) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    v->sync();
 #ifndef PG_HOSTSIM
-    v->stream = (stream == PGB200_PRIVATE_STREAM) ? v->own_stream : (cudaStream_t)stream;
+    cudaStream_t next = (stream == PGB200_PRIVATE_STREAM) ? v->own_stream : (cudaStream_t)stream;
+    // a stream that is capturing cannot be waited on, neither the new one nor the old one: moving into a
+    // capture, the caller has ordered the handle's earlier work before the capture began
+    if (!stream_capturing(next) && !v->capturing())
+        v->sync();
+    v->stream = next;
 #else
+    v->sync();
     (void)stream;
 #endif
 }
@@ -1039,6 +1096,8 @@ int pgb200_set_rgb_mirror(libenv_env *handle, void *mirror0, void *mirror1) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->sync();
     v->mirror[0] = (uint8_t *)mirror0;
     v->mirror[1] = (uint8_t *)(mirror1 ? mirror1 : mirror0);
@@ -1054,6 +1113,8 @@ int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int 
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->ensure_initial_reset();
     v->sync();
     if (buffer == nullptr || dtype == 0) {
@@ -1069,8 +1130,9 @@ int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int 
     v->base.consumer = buffer;
     v->base.consumer_lut = v->d_consumer_lut;
     v->base.consumer_k = k_frames;
-    v->base.consumer_slot = 0;
+    v->consumer_slot = 0;
     v->consumer_steps = 0;
+    CUDA_CHECK(cudaMemsetAsync(v->d_consumer_slot, 0, sizeof(int32_t), v->stream));
     // the current frame of every env becomes the newest frame of an otherwise empty stack
     for (size_t g = 0; g < v->games.size(); g++) {
         KParams p = v->base;
@@ -1098,13 +1160,44 @@ int pgb200_debug_phase_offset(void) {
 #endif
 }
 
-int pgb200_consumer_slot(libenv_env *handle) { return ((VecEnv *)handle)->base.consumer_slot; }
+int pgb200_consumer_slot(libenv_env *handle) { return ((VecEnv *)handle)->consumer_slot; }
+
+int pgb200_get_consumer_slot_device(libenv_env *handle, int32_t **out) {
+#ifndef PG_HOSTSIM
+    *out = ((VecEnv *)handle)->d_consumer_slot;
+    return 0;
+#else
+    (void)handle;
+    *out = nullptr;
+    return -1;
+#endif
+}
 
 int pgb200_mirror_parity(libenv_env *handle) { return ((VecEnv *)handle)->mirror_parity; }
 
 void pgb200_act_device(libenv_env *handle) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing()) {
+#ifndef PG_HOSTSIM
+        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+        if (cudaStreamIsCapturing(v->stream, &st) == cudaErrorStreamCaptureImplicit) {
+            cudaGetLastError();
+            pg_fatal("pgb200_act_device: a CUDA graph capture is running on another stream and the handle is on the legacy "
+                     "default stream; rebind it to the capturing stream first (pgb200_set_stream)\n");
+        }
+        if (v->timing)
+            pg_fatal("pgb200_act_device: a step under kernel timing cannot be captured\n");
+#endif
+        // what a captured step cannot contain: the initial reset, host-side state that changes from step to
+        // step (the mirror parity, the host buffers' copies) and the timing events
+        if (!v->initial_reset_done)
+            pg_fatal("pgb200_act_device: the initial reset cannot be captured; call pgb200_get_device_buffers first\n");
+        if (v->mirror[0])
+            pg_fatal("pgb200_act_device: a step with the peer mirror set cannot be captured\n");
+        if (v->have_host_bufs)
+            pg_fatal("pgb200_act_device: a handle with host buffers cannot be captured\n");
+    }
     v->ensure_initial_reset();
     v->launch(false);
 }
@@ -1112,12 +1205,15 @@ void pgb200_act_device(libenv_env *handle) {
 void pgb200_sync(libenv_env *handle) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    v->refuse_in_capture("pgb200_sync");
     v->sync();
 }
 
 uint32_t pgb200_get_errors(libenv_env *handle, uint32_t *host_out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return UINT32_MAX;
     v->sync();
     const size_t N = (size_t)v->num_envs;
     std::vector<EnvHdr> hdr(N);
@@ -1140,6 +1236,8 @@ int pgb200_debug_cycles(libenv_env *handle, uint32_t *host_out) {
     if (!v->base.dbg_cycles)
         return -1;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->sync();
 #ifndef PG_HOSTSIM
     CUDA_CHECK(cudaMemcpy(host_out, v->base.dbg_cycles, (size_t)v->num_envs * 4, cudaMemcpyDeviceToHost));
@@ -1150,6 +1248,8 @@ int pgb200_debug_cycles(libenv_env *handle, uint32_t *host_out) {
 int pgb200_debug_read_env(libenv_env *handle, int env, void *hdr_out, void *ents_out, int max_ents) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->sync();
     EnvHdr hdr;
     const KParams &p = v->base;
@@ -1210,6 +1310,8 @@ int get_state(libenv_env *handle, int env_idx, char *data, int length) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
     pg_fassert(env_idx >= 0 && env_idx < v->num_envs);
+    if (v->capturing())
+        return -1;
     v->ensure_initial_reset();
     v->sync();  // wait_for_stepping_threads
     host::HostEnv e;
@@ -1229,6 +1331,7 @@ void set_state(libenv_env *handle, int env_idx, char *data, int length) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
     pg_fassert(env_idx >= 0 && env_idx < v->num_envs);
+    v->refuse_in_capture("set_state");
     v->ensure_initial_reset();
     v->sync();
     host::HostEnv e;
@@ -1272,6 +1375,7 @@ int64_t pgb200_kernel_launches(libenv_env *handle) { return ((VecEnv *)handle)->
 void pgb200_set_launch_shape(libenv_env *handle, int chunks, int serialize) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    v->refuse_in_capture("pgb200_set_launch_shape");
     v->sync();
     v->force_chunks = chunks;
     v->serialize_launches = serialize != 0;
@@ -1281,6 +1385,8 @@ int pgb200_kernel_timing_begin(libenv_env *handle, int max_launch_pairs) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->sync();
     while ((int)v->tev_pool.size() < 4 * max_launch_pairs) {
         cudaEvent_t e;
@@ -1300,6 +1406,8 @@ int pgb200_kernel_timing_end(libenv_env *handle, double *out) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
+    if (v->capturing())
+        return -1;
     v->sync();
     v->timing = false;
     double logic_ms = 0, setup_ms = 0, render_ms = 0, envs = 0;

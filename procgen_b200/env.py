@@ -136,6 +136,10 @@ class BaseProcgenEnv:
         self._host_buffers = bool(host_buffers)
         self._torch = None
         self._next_level_seeds = None
+        self._consumer_slot = None
+        self._graph_stepped = False   # act() has run inside a CUDA graph capture
+        self._retired_consumers = []  # consumer buffers a captured graph may still write
+        self._timing = False
         if self._lib.pgb200_is_device_build():
             import torch
 
@@ -234,12 +238,52 @@ class BaseProcgenEnv:
     def observe(self):
         """-> (rew f32[N], {"rgb": u8[N,64,64,3]}, first bool[N]); device tensors unless host_buffers."""
         if self._host_buffers:
+            self._refuse_in_capture("observe")
             self._lib.libenv_observe(self._h)
             return self._rew, {"rgb": self._rgb}, self._first.astype(bool)
         return self._rew, {"rgb": self._rgb}, self._first.bool()
 
+    # ------------------------------------------------------------------ CUDA graph capture
+    def _capturing(self) -> bool:
+        return self._torch is not None and self._torch.cuda.is_current_stream_capturing()
+
+    def _refuse_in_capture(self, method: str) -> None:
+        if self._capturing():
+            raise RuntimeError(f"procgen_b200: {method}() cannot run inside CUDA graph capture (it waits for the GPU or "
+                               "allocates); call it before the capture or after it")
+
+    def _wait_for_replays(self) -> None:
+        """Before a call that reads or writes env state from the host: once this handle has been captured, its
+        steps may also be graph replays on the caller's current stream, which the handle's own stream does not
+        see. Rebinding to that stream waits for both."""
+        if self._graph_stepped and not self._host_buffers:
+            with self._torch.cuda.device(self._dev):
+                cur = self._torch.cuda.current_stream(self._dev).cuda_stream
+                self._lib.pgb200_set_stream(self._h, C.c_void_p(cur))
+                self._stream_handle = cur
+                self._lib.pgb200_sync(self._h)
+
     def act(self, ac):
-        """env.py:197-200: actions are cast to int32. Asynchronous, like VecGame::act."""
+        """env.py:197-200: actions are cast to int32. Asynchronous, like VecGame::act.
+
+        Inside ``torch.cuda.graph`` (or any capture on the current stream) act() takes a CUDA tensor only and
+        the step becomes part of the graph: the handle is rebound to the capture stream without a host wait,
+        and every replay steps the envs again with whatever the action tensor then holds. Set up before the
+        capture what the step should use (next_level_seeds(), enable_consumer_output(), set_launch_shape()):
+        a graph keeps the launch shape, the level choice and the consumer output it was captured with."""
+        if self._capturing():
+            if self._host_buffers:
+                raise RuntimeError("procgen_b200: act() cannot be captured in a CUDA graph with host_buffers=True; "
+                                   "use the device-resident handle")
+            if not (self._torch.is_tensor(ac) and ac.is_cuda):
+                raise RuntimeError("procgen_b200: act() inside CUDA graph capture takes a CUDA tensor of actions; "
+                                   "host arrays need a synchronised copy that cannot be captured")
+            if getattr(self, "_peer", None) is not None:
+                raise RuntimeError("procgen_b200: act() cannot be captured while enable_peer_gather() is on: the mirror "
+                                   "buffer alternates on the host")
+            if self._timing:
+                raise RuntimeError("procgen_b200: act() cannot be captured between kernel_timing_begin() and kernel_timing_end()")
+            self._graph_stepped = True
         if self._host_buffers:
             self._ac[:] = np.asarray(ac).astype(np.int32)
             if self._next_level_seeds is not None:
@@ -250,7 +294,8 @@ class BaseProcgenEnv:
             return
         torch = self._torch
         with torch.cuda.device(self._dev):
-            # keep every launch on the caller's current stream
+            # keep every launch on the caller's current stream (a capture stream included: the library rebinds
+            # to a capturing stream without waiting)
             cur = torch.cuda.current_stream(self._dev).cuda_stream
             if cur != self._stream_handle:
                 self._lib.pgb200_set_stream(self._h, C.c_void_p(cur))
@@ -279,6 +324,7 @@ class BaseProcgenEnv:
     def get_info(self) -> List[dict]:
         """gym3's list-of-dicts form (env.py:128-136). One D2H copy for all three columns; callers on
         the hot path should use get_info_tensors() (columns, no copy) instead."""
+        self._refuse_in_capture("get_info")
         if self._host_buffers:
             cols = [self._info[k].tolist() for k in self._info_names]
         else:
@@ -303,8 +349,12 @@ class BaseProcgenEnv:
         neither read nor change the array.
 
         Write it with torch ops on the stream you step on (device-resident mode); with host_buffers=True,
-        act() waits for the current torch stream before it starts the step."""
+        act() waits for the current torch stream before it starts the step.
+
+        A CUDA graph reads the array only if it was requested before the capture: call this once first. Inside
+        the capture the tensor may then be refilled with torch ops like any other input of the graph."""
         if self._next_level_seeds is None:
+            self._refuse_in_capture("next_level_seeds")
             torch = self._torch
             ptr = C.POINTER(C.c_int32)()
             with torch.cuda.device(self.device_index):
@@ -321,6 +371,8 @@ class BaseProcgenEnv:
         """One bytes blob per env in the reference's wire format (env.py:139-147, vecgame.cpp:437-445)."""
         import ctypes as C
 
+        self._refuse_in_capture("get_state")
+        self._wait_for_replays()
         buf = C.create_string_buffer(MAX_STATE_SIZE)
         out = []
         for i in range(self.num):
@@ -331,6 +383,8 @@ class BaseProcgenEnv:
     def set_state(self, states):
         """Load one blob per env (env.py:149-153, vecgame.cpp:447-457); observations and info are refreshed."""
         assert len(states) == self.num
+        self._refuse_in_capture("set_state")
+        self._wait_for_replays()
         for i, st in enumerate(states):
             self._lib.set_state(self._h, i, st, len(st))
 
@@ -355,28 +409,37 @@ class BaseProcgenEnv:
 
     # ------------------------------------------------------------------ GPU extras
     def sync(self):
+        self._refuse_in_capture("sync")
         self._lib.pgb200_sync(self._h)
 
     def errors(self) -> int:
         """OR of the per-env sticky error bits (0 = healthy)."""
+        self._refuse_in_capture("errors")
+        self._wait_for_replays()
         return int(self._lib.pgb200_get_errors(self._h, None))
 
     def kernel_launches(self) -> int:
+        """Kernel launches issued so far; a step captured in a CUDA graph counts once, not per replay."""
         return int(self._lib.pgb200_kernel_launches(self._h))
 
     def set_launch_shape(self, chunks: int = 0, serialize: bool = False) -> None:
         """Measurement knob (see pgb200_set_launch_shape): env chunks per step, launches back to back."""
+        self._refuse_in_capture("set_launch_shape")
         self._lib.pgb200_set_launch_shape(self._h, int(chunks), int(bool(serialize)))
 
     def kernel_timing_begin(self, max_launch_pairs: int) -> None:
         """Bracket every (logic, render) kernel pair with CUDA events until kernel_timing_end()."""
+        self._refuse_in_capture("kernel_timing_begin")
         self._lib.pgb200_kernel_timing_begin(self._h, int(max_launch_pairs))
+        self._timing = True
 
     def kernel_timing_end(self) -> dict:
         import ctypes as C
 
+        self._refuse_in_capture("kernel_timing_end")
         out = (C.c_double * 5)()
         pairs = int(self._lib.pgb200_kernel_timing_end(self._h, out))
+        self._timing = False
         return {"logic_ms": out[0], "render_ms": out[1], "setup_ms": out[4], "launch_pairs": pairs, "env_steps": out[3]}
 
     def enable_peer_gather(self, dst: int = 0) -> bool:
@@ -388,6 +451,7 @@ class BaseProcgenEnv:
         Returns False (and keeps the NCCL gather) when symmetric memory cannot be set up."""
         import torch.distributed as dist
 
+        self._refuse_in_capture("enable_peer_gather")
         torch = self._torch
         world, rank = dist.get_world_size(), dist.get_rank()
         ok = torch.zeros(1, device=self._dev, dtype=torch.int32)
@@ -442,11 +506,18 @@ class BaseProcgenEnv:
         """Have the render kernel also write what a learner feeds its network: rgb / 255 as float16 or
         bfloat16, planar CHW, `frames` frames stacked along the channel axis with baselines'
         VecFrameStack reset rule (an env that starts an episode sees zeros for the older frames).
-        consumer_observation() then returns [num, 3*frames, 64, 64] without any further kernel."""
+        consumer_observation() then returns [num, 3*frames, 64, 64] without any further kernel.
+
+        A CUDA graph keeps the buffer, dtype and frames it was captured with: enable the output before the
+        capture, and capture again after changing it."""
+        self._refuse_in_capture("enable_consumer_output")
         torch = self._torch
         dtype = dtype or torch.float16
         code = {torch.float16: 1, torch.bfloat16: 2}[dtype]
         slots = 1 if frames == 1 else 2 * frames
+        if self._graph_stepped and getattr(self, "_consumer", None) is not None:
+            # a graph captured earlier still writes the old buffer: never hand its memory to anything else
+            self._retired_consumers.append(self._consumer)
         with torch.cuda.device(self._dev):
             self._consumer = torch.zeros((self.num, slots, 3, 64, 64), dtype=dtype, device=self._dev)
             self._consumer_k = int(frames)
@@ -456,12 +527,48 @@ class BaseProcgenEnv:
             raise ValueError("pgb200_set_consumer_output rejected the arguments")
 
     def consumer_observation(self):
-        """[num, 3*frames, 64, 64] view (oldest frame first) of the consumer output; valid until the next act()."""
+        """[num, 3*frames, 64, 64] view (oldest frame first) of the consumer output; valid until the next act().
+
+        Once the handle has been stepped inside a CUDA graph, graph replays move the ring on the device only,
+        so from then on (and inside the capture) this is a copy gathered through consumer_slot_tensor(),
+        without a host wait, instead of a view."""
         k = self._consumer_k
         if k == 1:
             return self._consumer[:, 0]
+        if self._graph_stepped or self._capturing():
+            torch = self._torch
+            idx = self.consumer_slot_tensor().to(torch.int64) + 1 + torch.arange(k, device=self._dev)
+            return self._consumer.index_select(1, idx).reshape(self.num, 3 * k, 64, 64)
         s = int(self._lib.pgb200_consumer_slot(self._h))
         return self._consumer[:, s + 1:s + 1 + k].reshape(self.num, 3 * k, 64, 64)
+
+    def consumer_slot_tensor(self):
+        """int32 CUDA tensor [1] aliasing the device-resident ring position s of the consumer output: the slot the
+        latest step wrote, advanced on the device by every step, eager or replayed from a CUDA graph. The ordered
+        stack (oldest frame first) is ring slots s + 1 .. s + k of the [num, 2k, 3, 64, 64] ring (k > 1), so a
+        captured policy reads it without the host:
+
+            slot, ring = env.consumer_slot_tensor(), env.consumer_ring()   # before the capture
+            ar = torch.arange(k, device="cuda")
+            with torch.cuda.graph(g):
+                env.act(actions)
+                idx = slot.long() + 1 + ar
+                obs = ring.index_select(1, idx).reshape(env.num, 3 * k, 64, 64)
+                logits = policy(obs)
+
+        (consumer_observation() does the same once the handle has been captured.) Written on the stream the
+        handle steps on."""
+        if self._consumer_slot is None:
+            torch = self._torch
+            ptr = C.POINTER(C.c_int32)()
+            if self._lib.pgb200_get_consumer_slot_device(self._h, C.byref(ptr)) != 0:
+                raise RuntimeError("pgb200_get_consumer_slot_device failed")
+            self._consumer_slot = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (1,), "<i4"), device=self._dev)
+        return self._consumer_slot
+
+    def consumer_ring(self):
+        """The consumer output's ring itself: [num, slots, 3, 64, 64] (slots = 1 for frames == 1, else 2 * frames)."""
+        return self._consumer
 
     def gather_how(self) -> str:
         if getattr(self, "_peer", None) is not None:

@@ -49,7 +49,8 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_sync", "pgb200_get_errors", "pgb200_debug_cycles", "pgb200_debug_read_env", "pgb200_kernel_launches", "pgb200_is_device_build",
            "pgb200_kernel_timing_begin", "pgb200_kernel_timing_end", "get_state", "set_state", "pgb200_set_launch_shape",
            "pgb200_frame_info", "pgb200_set_rgb_mirror", "pgb200_mirror_parity",
-           "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds"]
+           "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
+           "pgb200_get_consumer_slot_device"]
 
 _lib = None
 
@@ -85,6 +86,8 @@ def bind(lib):
     lib.pgb200_set_consumer_output.restype = C.c_int
     lib.pgb200_consumer_slot.argtypes = [C.c_void_p]
     lib.pgb200_consumer_slot.restype = C.c_int
+    lib.pgb200_get_consumer_slot_device.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
+    lib.pgb200_get_consumer_slot_device.restype = C.c_int
     lib.pgb200_mirror_parity.argtypes = [C.c_void_p]
     lib.pgb200_mirror_parity.restype = C.c_int
     lib.pgb200_kernel_launches.argtypes = [C.c_void_p]
