@@ -171,6 +171,39 @@ LIBENV_API int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_devic
  * action buffer; with libenv_act, the writes must be complete before the call. Returns 0. */
 LIBENV_API int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out);
 
+/* Final outputs: the frame each env's level ended in, and why it ended. A step that ends an episode resets
+ * the env inside it and returns the next level's first frame (Game::step, game.cpp:120-155); these arrays
+ * keep what that reset hides, e.g. the state V(s_T) of a truncated episode is computed on.
+ *   rgb        [num_envs][64][64][3] uint8
+ *   level_end  [num_envs] uint8
+ * Device memory (host memory in the CPU debug build), also for a handle with host buffers: there the arrays
+ * are complete once libenv_observe returns. The first call allocates them, zero-filled, performs the
+ * initial reset if it has not happened yet and returns 0; from then on every step of the handle fills them
+ * (there is no off switch). The pointers stay valid until libenv_close.
+ * After every step, level_end[e] says whether env e's level was reset inside that step, and why, in the
+ * order the reference tests it (game.cpp:132-134):
+ *   0                          no reset; rgb[e] is left as it was
+ *   PGB200_LEVEL_END_GAME      the game ended the level: the agent died or completed it (prev_level_complete
+ *                              tells which)
+ *   PGB200_LEVEL_END_TIMEOUT   the game did not, but the episode reached its step limit (a truncation)
+ *   PGB200_LEVEL_END_CALLER    neither: the reset came from action -1
+ * and where it is not 0, rgb[e] is the frame Game::observe would have rendered had the step not reset.
+ * level_end[e] != 0 exactly where first[e] == 1, with one exception: under use_sequential_levels a
+ * completed level resets with first = 0 (game.cpp:148-150) and reports PGB200_LEVEL_END_GAME.
+ * Every other output of the step (rgb, rew, first, the infos, the consumer output, next_level_seed
+ * consumption, the state) is what it is without this call. The initial reset, get_state and set_state
+ * neither read nor write the arrays. CUDA graphs: the first call is refused (-1) while the handle's stream
+ * captures; a captured step keeps whether final outputs were on at capture.
+ * pgb200_kernel_timing_begin returns -1 on a handle with final outputs. */
+#define PGB200_LEVEL_END_GAME 1
+#define PGB200_LEVEL_END_TIMEOUT 2
+#define PGB200_LEVEL_END_CALLER 3
+struct pgb200_final_outputs {
+    uint8_t *rgb;        /* [num_envs][64][64][3] */
+    uint8_t *level_end;  /* [num_envs] */
+};
+LIBENV_API int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *out);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -266,7 +299,8 @@ LIBENV_API int64_t pgb200_kernel_launches(libenv_env *handle);
  * runs on. end() synchronises and writes out[0] = sum of logic-kernel ms, out[1] = sum of render-kernel
  * ms, out[2] = number of launch triples timed, out[3] = env-steps those launches processed, out[4] =
  * sum of setup-kernel ms (out must hold 5 doubles); returns the number of triples. At most
- * max_launch_pairs triples are timed (further launches run untimed). */
+ * max_launch_pairs triples are timed (further launches run untimed). Returns -1 on a handle with final
+ * outputs (pgb200_get_final_outputs): the second phase of its steps is not bracketed by the triples. */
 LIBENV_API int pgb200_kernel_timing_begin(libenv_env *handle, int max_launch_pairs);
 /* Measurement knob: chunks > 0 forces that many env chunks per game and step (0 = the default
  * policy); serialize != 0 keeps every launch on the handle's stream, back to back, so a kernel's

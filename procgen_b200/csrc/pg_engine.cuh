@@ -821,7 +821,10 @@ struct Engine {
     // (the reset of an episode that just ended) as a separate pass: step_play = everything up to the
     // decision `if (step_data.done) reset()`, returns that decision; step_finish = the rest, returns whether
     // its reset took level_seed_override.
-    static PG_HD bool step_play(Ctx &c) {
+    // level_end (pgb200_get_final_outputs): receives why the level ends in this step, in the order of the
+    // `done` expression below: PGB200_LEVEL_END_GAME, _TIMEOUT, _CALLER, or 0 when it does not end.
+    template <bool CAUSE = false>
+    static PG_HD bool step_play(Ctx &c, uint8_t *level_end = nullptr) {
         EnvHdr &h = *c.h;
         h.cur_time += 1;
         bool will_force_reset = false;
@@ -833,6 +836,8 @@ struct Engine {
         h.done = 0;
         h.level_complete = 0;
         G::game_step(c);
+        if (CAUSE)
+            *level_end = h.done ? 1 : (h.cur_time >= h.timeout ? 2 : (will_force_reset ? 3 : 0));
         h.done = h.done || will_force_reset || (h.cur_time >= h.timeout);
         h.total_reward += h.reward;
         if (h.reward != 0) {

@@ -55,6 +55,12 @@ struct KParams {
     int32_t consumer_k;         // frames per stack; slots = k == 1 ? 1 : 2k
     const int32_t *consumer_slot_dev;  // device: ring position this step writes, t mod k (advanced on the device once per step)
     uint32_t *dbg_cycles;       // optional [N] per-env logic duration in SM cycles (profiling aid)
+    // optional final outputs (pgb200_get_final_outputs); null = off. A step then runs in two phases per launch:
+    // A renders the final state of the envs whose level ends, B resets exactly those (reset_list) and renders again
+    uint8_t *final_rgb;         // [N][64][64][3]
+    uint8_t *level_end;         // [N] why env's level ended in this step (PGB200_LEVEL_END_*), 0 = it did not
+    int32_t *reset_list;        // this launch's own segment of an [N] list: the envs phase B resets
+    unsigned int *reset_count;  // entries in reset_list (device; beside the launch's ticket)
 };
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
@@ -166,6 +172,40 @@ PG_HD void env_step_logic(const KParams &p, int env) {
     } else {
         Engine<G>::step(c);
     }
+    Raster<G, Frame>::prepare_camera(c);
+    write_step_outputs(p, env, *c.h);
+}
+
+// Phase A of a step with final outputs: Game::step up to the reset decision, with the cause of a level end
+// in level_end[env]. An env that does not reset finishes as in env_step_logic. One that does gets the camera
+// of its final state, and the rest of its step (the reset and the scalar outputs) waits for phase B,
+// env_finish_logic. Returns whether the env resets.
+template <class G, class Frame>
+PG_HD bool env_step_logic_final(const KParams &p, int env) {
+#if defined(__CUDA_ARCH__)
+    env_prefetch(p, env);
+#endif
+    Ctx c = make_ctx(p, env);
+    c.h->action = p.action[env];  // vecgame.cpp:388
+    uint8_t cause = 0;
+    const bool do_reset = Engine<G>::template step_play<true>(c, &cause);
+    p.level_end[env] = cause;
+    if (!do_reset)
+        Engine<G>::step_finish(c, false, -1);
+    Raster<G, Frame>::prepare_camera(c);
+    if (!do_reset)
+        write_step_outputs(p, env, *c.h);
+    return do_reset;
+}
+
+// Phase B: the rest of Game::step for an env whose level ended in phase A. The reset reads and consumes the
+// env's next_level_seed entry as env_step_logic<LEVEL_CHOICE> does; then Game::observe's camera and scalars.
+template <class G, class Frame>
+PG_HD void env_finish_logic(const KParams &p, int env) {
+    Ctx c = make_ctx(p, env);
+    const int32_t next_seed = p.next_level_seed ? p.next_level_seed[env] : -1;
+    if (Engine<G>::step_finish(c, true, next_seed))
+        p.next_level_seed[env] = -1;
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, *c.h);
 }

@@ -69,7 +69,8 @@ constexpr int kRenderThreads = 128;
 // Persistent: the grid is sized to fill the machine once and every warp pulls env indices from a
 // global ticket counter until the launch's range is exhausted, so a long env (level reset) only
 // delays its own warp and no SM slot idles waiting for a block launch.
-template <class G, bool INIT, bool LEVEL_CHOICE = false>
+// FINAL: phase A of a step with final outputs; an env whose level ends is appended to p.reset_list.
+template <class G, bool INIT, bool LEVEL_CHOICE = false, bool FINAL = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -84,11 +85,33 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
         const long long t0 = p.dbg_cycles ? clock64() : 0;
         if (INIT)
             env_init_logic<G, Frame>(p, env);
-        else
+        else if (FINAL) {
+            if (env_step_logic_final<G, Frame>(p, env) && lane == 0)
+                p.reset_list[atomicAdd(p.reset_count, 1u)] = env;
+        } else
             env_step_logic<G, Frame, LEVEL_CHOICE>(p, env);
         __syncwarp();
         if (p.dbg_cycles && lane == 0)
             p.dbg_cycles[env] = (uint32_t)(clock64() - t0);
+    }
+}
+
+// Phase B of a step with final outputs: the resets of the envs phase A listed. Persistent and ticketed like the
+// logic kernel, because level generation runs here (milliseconds for caveflyer, jumper and leaper).
+template <class G>
+__global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_kernel(KParams p, unsigned int *ticket) {
+    using Frame = typename FrameFor<G>::type;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned count = *p.reset_count;
+    while (true) {
+        unsigned t = 0;
+        if (lane == 0)
+            t = atomicAdd(ticket, 1u);
+        t = __shfl_sync(0xffffffffu, t, 0);
+        if (t >= count)
+            break;
+        env_finish_logic<G, Frame>(p, p.reset_list[t]);
+        __syncwarp();
     }
 }
 
@@ -101,10 +124,20 @@ constexpr int kSetupThreads = 128;
 #ifndef PG_SETUP_MIN_BLOCKS
 #define PG_SETUP_MIN_BLOCKS 8   // 64 registers x 32 warps/SM: more envs in flight beat more registers (96 x 20 was slower)
 #endif
-template <class G, int VIEW>
+// LIST: phase B of a step with final outputs, the warps of the grid stride over p.reset_list
+template <class G, int VIEW, bool LIST = false>
 __global__ void __launch_bounds__(kSetupThreads, PG_SETUP_MIN_BLOCKS) setup_kernel(KParams p) {
     using Setup = typename FrameFor<G, VIEW>::setup;
     const int i = (int)blockIdx.x * (kSetupThreads / 32) + (int)(threadIdx.x >> 5);
+    if (LIST) {
+        const int count = (int)*p.reset_count;
+        for (int j = i; j < count; j += (int)gridDim.x * (kSetupThreads / 32)) {
+            const int env = p.reset_list[j];
+            Setup &f = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
+            env_setup_frame<G, Setup>(p, env, f, (int)(threadIdx.x & 31u), 32);
+        }
+        return;
+    }
     if (i >= p.env_count)
         return;
     const int env = p.env_first + i * p.env_step;
@@ -175,12 +208,12 @@ __device__ __forceinline__ void pg_bulk_store_and_wait(void *dst_gmem, const voi
 //   compose                warp w owns rows y = w (mod 4): gather (cells over background; a lane = 4 pixel
 //                          columns x 8 rows), then paint the entity blits in draw order, lanes sharing each blit
 //   pack + store           RGB32 -> RGB888 in place, one bulk copy of the 12 KiB frame to the observation buffer
-template <class G, int VIEW>
-__global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlocks) render_kernel(KParams p) {
+// render_env_frame is that sequence for the env env_of() returns, on mbarrier phase `parity`. PASS: see
+// render_kernel. The env index and whether phase A's env ended its level are fetched where they are needed, so
+// that nothing stays live across the frame (the 8-CTA games have no register to spare).
+template <class G, int VIEW, int PASS, class EnvOf>
+__device__ __forceinline__ void render_env_frame(const KParams &p, typename FrameFor<G, VIEW>::type &f, EnvOf env_of, unsigned parity) {
     using Frame = typename FrameFor<G, VIEW>::type;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    Frame &f = *reinterpret_cast<Frame *>(smem_raw);
-    const int env = p.env_first + (int)blockIdx.x * p.env_step;
     const int tid = (int)threadIdx.x;
 #ifdef PG_PHASE_TIMING
     long long t0 = clock64(), t1;
@@ -188,7 +221,7 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
     do {                                                          \
         t1 = clock64();                                           \
         if (tid == 0)                                             \
-            p.hdr[env].dbg_phase[id] = (uint32_t)(t1 - t0);       \
+            p.hdr[env_of()].dbg_phase[id] = (uint32_t)(t1 - t0);       \
         t0 = t1;                                                  \
     } while (0)
 #else
@@ -196,10 +229,7 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
 #endif
     using Shared = typename FrameFor<G, VIEW>::shared;
     using Setup = typename FrameFor<G, VIEW>::setup;
-    const Setup *gs = reinterpret_cast<const Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
-    if (tid == 0)
-        pg_mbar_init(&f.mbar, 1);
-    __syncthreads();
+    const Setup *gs = reinterpret_cast<const Setup *>(p.frame_setup + (size_t)env_of() * p.frame_setup_stride);
     if (tid < 32) {
         // Everything the setup kernel prepared for this env — one bulk copy into the head of the frame —
         // and the pre-scaled tiles its cells need, one bulk copy each, all counted on one mbarrier phase.
@@ -215,19 +245,19 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
         for (int j = tid; j < nj; j += 32)
             pg_bulk_load(f.arena + gs->tjob_dst[j], p.tiles.texels + gs->tjob_src[j], 4u * gs->tjob_words[j], &f.mbar);
     }
-    pg_mbar_wait(&f.mbar, 0);
+    pg_mbar_wait(&f.mbar, parity);
     PG_RENDER_PHASE(0);
     // warp w owns rows y = w (mod warps): gather and paint need no block barrier in between
     env_render_compose<G, Frame>(p, f, tid >> 5, kRenderThreads >> 5, tid & 31, 32);
     __syncthreads();
     PG_RENDER_PHASE(5);
-    if (p.consumer != nullptr) {
+    if (p.consumer != nullptr && !(PASS == 1 && p.level_end[env_of()] != 0)) {
         // Consumer epilogue: the frame as normalised 16-bit floats, planar, into ring slot s (and its
         // twin s + k); an env that starts an episode this step gets the older frames of its window
         // zeroed (the frame-stack convention of baselines' VecFrameStack). Thread = pixel pairs.
         const int kf = p.consumer_k, s = *p.consumer_slot_dev;
         const int slots = kf == 1 ? 1 : 2 * kf;
-        uint32_t *base = reinterpret_cast<uint32_t *>(p.consumer) + (size_t)env * slots * (3 * RES_W * RES_H / 2);
+        uint32_t *base = reinterpret_cast<uint32_t *>(p.consumer) + (size_t)env_of() * slots * (3 * RES_W * RES_H / 2);
         const uint16_t *lut = p.consumer_lut;
         for (int pair = tid; pair < RES_W * RES_H / 2; pair += kRenderThreads) {
             const uint32_t c0 = f.fb[2 * pair], c1 = f.fb[2 * pair + 1];
@@ -240,7 +270,7 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
                     base[(size_t)((s + kf) * 3 + ch) * (RES_W * RES_H / 2) + pair] = v;
             }
         }
-        if (kf > 1 && p.first[env]) {
+        if (kf > 1 && p.first[env_of()]) {
             // window of this step = ring slots s+1 .. s+k (the newest is s+k); zero the k-1 older ones
             // wherever they live: slot j and its twin j +- k
             for (int j = 1; j < kf; j++) {
@@ -269,9 +299,41 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
     __syncthreads();
     PG_RENDER_PHASE(6);
     if (tid == 0)
-        pg_bulk_store_and_wait(p.rgb + (size_t)env * (RES_W * RES_H * 3), f.fb, RES_W * RES_H * 3);
+        pg_bulk_store_and_wait((PASS == 1 && p.level_end[env_of()] != 0 ? p.final_rgb : p.rgb) + (size_t)env_of() * (RES_W * RES_H * 3), f.fb,
+                               RES_W * RES_H * 3);
     PG_RENDER_PHASE(7);
 #undef PG_RENDER_PHASE
+}
+
+// PASS 0: a plain step, one CTA per env of the launch. With final outputs (pgb200_get_final_outputs):
+// PASS 1 (phase A), the same grid, but the frame of an env whose level ended is its final frame: it goes to
+// final_rgb and skips the consumer epilogue, whose episode-start rule would read the previous step's first[env].
+// PASS 2 (phase B), a fixed grid whose CTAs loop over the envs phase A listed, after their reset: the mbarrier is
+// re-armed per env with alternating parity, and the bulk store's wait_group.read 0 has already released the frame.
+template <class G, int VIEW, int PASS = 0>
+__global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlocks) render_kernel(KParams p) {
+    using Frame = typename FrameFor<G, VIEW>::type;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    Frame &f = *reinterpret_cast<Frame *>(smem_raw);
+    if (threadIdx.x == 0)
+        pg_mbar_init(&f.mbar, 1);
+    __syncthreads();
+    if (PASS == 2) {
+        // the list entry is kept in shared memory and the count re-read each round
+        __shared__ int list_env;
+        for (unsigned i = 0;; i++) {
+            const int j = (int)(blockIdx.x + i * gridDim.x);
+            if (j >= (int)*p.reset_count)
+                break;
+            if (threadIdx.x == 0)
+                list_env = p.reset_list[j];
+            __syncthreads();
+            render_env_frame<G, VIEW, PASS>(p, f, [&] { return list_env; }, i & 1u);
+            __syncthreads();
+        }
+        return;
+    }
+    render_env_frame<G, VIEW, PASS>(p, f, [&] { return p.env_first + (int)blockIdx.x * p.env_step; }, 0);
 }
 
 #endif
@@ -311,6 +373,7 @@ struct LaunchCtx {
     cudaEvent_t link;
     unsigned int *ticket;     // work counter of this launch slot (one per in-flight logic kernel)
     int max_logic_blocks;     // SM count x resident CTAs per SM
+    int num_sms;              // SM count: sizes the machine-filling grids of a final-outputs step's phase B
     int render_smem_floor;    // dynamic shared memory requested per render CTA is at least this (co-residency knob)
     cudaEvent_t *tev;         // optional: 4 events (before logic, after it, after setup, after render) for kernel timing
 #endif
@@ -320,7 +383,7 @@ struct LaunchCtx {
 #ifndef PG_HOSTSIM
 // Dynamic shared memory of one render CTA (frame, or the co-residency floor) with the kernel's
 // opt-in limit raised to it once.
-template <class G, int VIEW>
+template <class G, int VIEW, int PASS = 0>
 int prepare_render_smem(const LaunchCtx &lc) {
     using Frame = typename FrameFor<G, VIEW>::type;
     const int bytes = (int)sizeof(Frame) > lc.render_smem_floor ? (int)sizeof(Frame) : lc.render_smem_floor;
@@ -330,10 +393,40 @@ int prepare_render_smem(const LaunchCtx &lc) {
     CUDA_CHECK(cudaGetDevice(&dev));
     int &have = attr_set[dev & 63];
     if (have < bytes) {
-        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
         have = bytes;
     }
     return bytes;
+}
+#endif
+
+#ifndef PG_HOSTSIM
+// One (game, env chunk) launch of a step with final outputs: two phases on the chunk's stream.
+//   A  logic (FINAL: listing the envs whose level ends), setup, render (their frames to final_rgb)
+//   B  finish (their resets), setup and render over the list: their next level's first frame to rgb
+// ticket[0] is phase A's ticket, ticket[1] the list's count and ticket[2] phase B's ticket: one memset clears
+// all three. Phase B's grids are fixed (machine-filling) and read the count on the device, so nothing waits for
+// the host and the step stays capturable. Everything goes to lc.stream (a priority-split logic stream would
+// let the next launch that shares this ticket slot clear it under phase B).
+template <class G, int VIEW>
+void launch_final_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
+    KParams q = p;
+    q.reset_count = lc.ticket + 1;
+    const int render_a = prepare_render_smem<G, VIEW, 1>(lc);
+    const int render_b = prepare_render_smem<G, VIEW, 2>(lc);
+    const int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
+    const int setup_b = setup_blocks < lc.num_sms * PG_SETUP_MIN_BLOCKS ? setup_blocks : lc.num_sms * PG_SETUP_MIN_BLOCKS;
+    const int render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
+    const int render_blocks_b = p.env_count < render_fit ? p.env_count : render_fit;
+    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, 3 * sizeof(unsigned int), lc.stream));
+    logic_kernel<G, false, false, true><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
+    setup_kernel<G, VIEW><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(q);
+    render_kernel<G, VIEW, 1><<<p.env_count, kRenderThreads, render_a, lc.stream>>>(q);
+    finish_kernel<G><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
+    setup_kernel<G, VIEW, true><<<setup_b, kSetupThreads, 0, lc.stream>>>(q);
+    render_kernel<G, VIEW, 2><<<render_blocks_b, kRenderThreads, render_b, lc.stream>>>(q);
+    CUDA_CHECK(cudaGetLastError());
+    (*lc.launch_counter) += 6;
 }
 #endif
 
@@ -351,6 +444,10 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     int logic_blocks = (p.env_count + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
     if (logic_blocks > lc.max_logic_blocks)
         logic_blocks = lc.max_logic_blocks;
+    if (!INIT && p.level_end) {
+        launch_final_step<G, VIEW>(p, lc, logic_blocks);
+        return;
+    }
     cudaStream_t ls = lc.logic_stream ? lc.logic_stream : lc.stream;
     CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, sizeof(unsigned int), ls));
     if (lc.tev)
@@ -375,6 +472,27 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     (*lc.launch_counter) += 3;
 #else
     static thread_local Frame *f = new Frame;
+    if (!INIT && p.level_end) {
+        // the serial twin of launch_final_step's two phases
+        unsigned int count = 0;
+        KParams q = p;
+        q.reset_count = &count;
+        KParams fin = q;
+        fin.rgb = p.final_rgb;
+        for (int b = 0; b < p.env_count; b++) {
+            const int env = p.env_first + b * p.env_step;
+            const bool ended = env_step_logic_final<G, Frame>(q, env);
+            if (ended)
+                q.reset_list[count++] = env;
+            render_env_serial<G, VIEW, Frame>(ended ? fin : q, env, *f);
+        }
+        for (unsigned int j = 0; j < count; j++) {
+            env_finish_logic<G, Frame>(q, q.reset_list[j]);
+            render_env_serial<G, VIEW, Frame>(q, q.reset_list[j], *f);
+        }
+        (*lc.launch_counter) += 6;
+        return;
+    }
     for (int b = 0; b < p.env_count; b++) {
         int env = p.env_first + b * p.env_step;
         if (INIT)

@@ -241,6 +241,8 @@ struct VecEnv {
     uint32_t *d_lvl_seeds = nullptr;
     int32_t *d_action = nullptr;
     int32_t *d_next_level_seed = nullptr;   // allocated by the first pgb200_get_next_level_seeds
+    // allocated by the first pgb200_get_final_outputs: base.final_rgb, base.level_end and the pending-reset list
+    int32_t *d_reset_list = nullptr;
     bool initial_reset_done = false;
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
@@ -266,9 +268,12 @@ struct VecEnv {
     static constexpr int kChunks = PG_STEP_CHUNKS;
     int force_chunks = 0;            // measurement knobs (pgb200_set_launch_shape)
     bool serialize_launches = false;
-    static constexpr int kMaxTickets = 64;   // launch slots in flight (one ticket counter each)
+    static constexpr int kMaxTickets = 64;   // launch slots in flight
+    // words per slot: the logic kernel's ticket; with final outputs also the pending-reset count and phase B's ticket
+    static constexpr int kTicketWords = 4;
     unsigned int *d_tickets = nullptr;
     int max_logic_blocks = 1 << 30;
+    int num_sms = 1;
     int render_smem_floor = 0;
     // host-buffer (libenv) mode
     // peer mirror (config 5, SURVEY §8e): when set, every launch's frames are also copied into
@@ -304,6 +309,7 @@ struct VecEnv {
         lc.link = nullptr;
         lc.ticket = d_tickets;
         lc.max_logic_blocks = max_logic_blocks;
+        lc.num_sms = num_sms;
         lc.render_smem_floor = render_smem_floor;
         lc.tev = nullptr;
 #endif
@@ -359,6 +365,8 @@ struct VecEnv {
                 p.env_first = g + lo * G;
                 p.env_step = G;
                 p.env_count = hi - lo;
+                if (base.reset_list)
+                    p.reset_list = base.reset_list + g * per_game + lo;  // the launch's own segment
                 LaunchCtx lc = lctx();
 #ifndef PG_HOSTSIM
                 if (nstreams) {
@@ -368,8 +376,8 @@ struct VecEnv {
                         lc.link = ev_link[k % nstreams];
                     }
                 }
-                lc.ticket = d_tickets + (k % kMaxTickets);
-                if (timing && tev_used + 4 <= tev_pool.size()) {
+                lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
+                if (timing && !base.level_end && tev_used + 4 <= tev_pool.size()) {
                     lc.tev = &tev_pool[tev_used];
                     tev_used += 4;
                     tev_envs.push_back(p.env_count);
@@ -636,6 +644,7 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
         cudaDeviceProp prop;
         CUDA_CHECK(cudaGetDeviceProperties(&prop, v->device));
         v->max_logic_blocks = prop.multiProcessorCount * PG_LOGIC_MIN_BLOCKS;
+        v->num_sms = prop.multiProcessorCount;
         // tuning knobs (defaults chosen by sweeping them with bench.py): resident logic blocks and
         // render CTAs per SM
         if (const char *e = getenv("PGB200_LOGIC_BLOCKS_PER_SM"))
@@ -649,7 +658,7 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
             v->render_smem_floor = (227 * 1024) / render_ctas - 1024 - 16;
             v->render_smem_floor &= ~15;
         }
-        CUDA_CHECK(cudaMalloc((void **)&v->d_tickets, VecEnv::kMaxTickets * sizeof(unsigned int)));
+        CUDA_CHECK(cudaMalloc((void **)&v->d_tickets, VecEnv::kMaxTickets * VecEnv::kTicketWords * sizeof(unsigned int)));
         v->d_consumer_slot = dev_alloc<int32_t>(1);
         v->base.consumer_slot_dev = v->d_consumer_slot;
     }
@@ -979,6 +988,9 @@ void libenv_close(libenv_env *handle) {
     dev_free(v->d_tile_sprites);
     dev_free(v->d_action);
     dev_free(v->d_next_level_seed);
+    dev_free(p.final_rgb);
+    dev_free(p.level_end);
+    dev_free(v->d_reset_list);
     dev_free(p.rgb);
     dev_free(p.rew);
     dev_free(p.first);
@@ -1073,6 +1085,35 @@ int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out) {
         v->base.next_level_seed = v->d_next_level_seed;
     }
     *out = v->d_next_level_seed;
+    return 0;
+}
+
+int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    if ((!v->initial_reset_done || !v->base.level_end) && v->capturing())
+        return -1;
+    v->ensure_initial_reset();
+    if (!v->base.level_end) {
+        const size_t N = (size_t)v->num_envs ? (size_t)v->num_envs : 1;
+        const size_t frames = N * RES_W * RES_H * 3;
+#ifndef PG_HOSTSIM
+        CUDA_CHECK(cudaMalloc((void **)&v->base.final_rgb, frames));
+        CUDA_CHECK(cudaMalloc((void **)&v->base.level_end, N));
+        CUDA_CHECK(cudaMalloc((void **)&v->d_reset_list, N * sizeof(int32_t)));
+        CUDA_CHECK(cudaMemsetAsync(v->base.final_rgb, 0, frames, v->stream));
+        CUDA_CHECK(cudaMemsetAsync(v->base.level_end, 0, N, v->stream));
+        // complete before the caller reads, from whatever stream it reads on
+        v->sync();
+#else
+        v->base.final_rgb = (uint8_t *)calloc(frames, 1);
+        v->base.level_end = (uint8_t *)calloc(N, 1);
+        v->d_reset_list = (int32_t *)calloc(N, sizeof(int32_t));
+#endif
+        v->base.reset_list = v->d_reset_list;
+    }
+    out->rgb = v->base.final_rgb;
+    out->level_end = v->base.level_end;
     return 0;
 }
 
@@ -1385,7 +1426,7 @@ int pgb200_kernel_timing_begin(libenv_env *handle, int max_launch_pairs) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing())
+    if (v->capturing() || v->base.level_end)
         return -1;
     v->sync();
     while ((int)v->tev_pool.size() < 4 * max_launch_pairs) {

@@ -136,6 +136,7 @@ class BaseProcgenEnv:
         self._host_buffers = bool(host_buffers)
         self._torch = None
         self._next_level_seeds = None
+        self._final_outputs = None
         self._consumer_slot = None
         self._graph_stepped = False   # act() has run inside a CUDA graph capture
         self._retired_consumers = []  # consumer buffers a captured graph may still write
@@ -364,6 +365,32 @@ class BaseProcgenEnv:
                 self._next_level_seeds = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "<i4"), device=dev)
         return self._next_level_seeds
 
+    def final_outputs(self):
+        """{"rgb": uint8 [num, 64, 64, 3], "level_end": uint8 [num]}: CUDA tensors aliasing the library's final
+        outputs (allocated, zero-filled, on the first call; from then on every step fills them). A step that ends
+        an episode resets the env inside it and returns the next level's first frame; after every step,
+        level_end[e] says whether env e's level ended in it and why: 0 it did not, 1 (LEVEL_END_GAME) the game
+        ended it (death or completion; prev_level_complete tells which), 2 (LEVEL_END_TIMEOUT) the step limit,
+        a truncation whose final state a learner bootstraps from, 3 (LEVEL_END_CALLER) action -1. Where
+        level_end[e] != 0, rgb[e] is the frame of the state the level ended in; elsewhere it keeps its value.
+        level_end != 0 exactly where first is set, except that under use_sequential_levels a completed level
+        continues with first = 0 and reports 1. Everything else the step outputs is unchanged.
+
+        A CUDA graph fills them only if they were requested before the capture: call this once first."""
+        if self._final_outputs is None:
+            self._refuse_in_capture("final_outputs")
+            torch = self._torch
+            out = L.FinalOutputs()
+            with torch.cuda.device(self.device_index):
+                if self._lib.pgb200_get_final_outputs(self._h, C.byref(out)) != 0:
+                    raise RuntimeError("pgb200_get_final_outputs failed")
+                dev = torch.device("cuda", self.device_index)
+                self._final_outputs = {
+                    "rgb": torch.as_tensor(_CudaArray(out.rgb, (self.num, 64, 64, 3), "|u1"), device=dev),
+                    "level_end": torch.as_tensor(_CudaArray(out.level_end, (self.num,), "|u1"), device=dev),
+                }
+        return dict(self._final_outputs)
+
     def callmethod(self, method: str, *args, **kwargs):
         return getattr(self, method)(*args, **kwargs)
 
@@ -430,7 +457,8 @@ class BaseProcgenEnv:
     def kernel_timing_begin(self, max_launch_pairs: int) -> None:
         """Bracket every (logic, render) kernel pair with CUDA events until kernel_timing_end()."""
         self._refuse_in_capture("kernel_timing_begin")
-        self._lib.pgb200_kernel_timing_begin(self._h, int(max_launch_pairs))
+        if self._lib.pgb200_kernel_timing_begin(self._h, int(max_launch_pairs)) != 0:
+            raise RuntimeError("procgen_b200: kernel timing is not available on a handle with final_outputs()")
         self._timing = True
 
     def kernel_timing_end(self) -> dict:
@@ -586,6 +614,7 @@ class BaseProcgenEnv:
             self._peer = None
         if getattr(self, "_h", None):
             self._next_level_seeds = None
+            self._final_outputs = None
             self._lib.libenv_close(self._h)
             self._h = None
 

@@ -38,6 +38,13 @@ class Buffers(C.Structure):
                 ("info", C.POINTER(C.c_void_p)), ("ac", C.POINTER(C.c_void_p))]
 
 
+class FinalOutputs(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("level_end", C.c_void_p)]
+
+
+LEVEL_END_GAME, LEVEL_END_TIMEOUT, LEVEL_END_CALLER = 1, 2, 3   # include/procgen_b200.h PGB200_LEVEL_END_*
+
+
 class DeviceBuffers(C.Structure):
     _fields_ = [("rgb", C.c_void_p), ("rew", C.c_void_p), ("first", C.c_void_p), ("prev_level_seed", C.c_void_p),
                 ("prev_level_complete", C.c_void_p), ("level_seed", C.c_void_p), ("action", C.c_void_p),
@@ -50,7 +57,7 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_kernel_timing_begin", "pgb200_kernel_timing_end", "get_state", "set_state", "pgb200_set_launch_shape",
            "pgb200_frame_info", "pgb200_set_rgb_mirror", "pgb200_mirror_parity",
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
-           "pgb200_get_consumer_slot_device"]
+           "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs"]
 
 _lib = None
 
@@ -70,6 +77,8 @@ def bind(lib):
     lib.pgb200_get_device_buffers.restype = C.c_int
     lib.pgb200_get_next_level_seeds.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
     lib.pgb200_get_next_level_seeds.restype = C.c_int
+    lib.pgb200_get_final_outputs.argtypes = [C.c_void_p, C.POINTER(FinalOutputs)]
+    lib.pgb200_get_final_outputs.restype = C.c_int
     lib.pgb200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     lib.pgb200_set_stream.restype = None
     lib.pgb200_get_errors.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
