@@ -204,6 +204,30 @@ struct pgb200_final_outputs {
 };
 LIBENV_API int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *out);
 
+/* Per-env pause: `*out` = this handle's uint8 array pause[num_envs] (device memory; host memory in the CPU
+ * debug build), allocated and filled with 0 by the first call, which also performs the initial reset if it has
+ * not happened yet. Returns 0. The pointer stays valid until libenv_close. A step does not consume an entry:
+ * it stays in force until the caller clears it. In every step, an env e with pause[e] != 0 is paused:
+ *   - its state is untouched, byte for byte (both RNGs, cur_time: a paused step does not count toward the time
+ *     limit, the entities, the grid), and its action, -1 included, is ignored;
+ *   - its next_level_seed entry is neither read nor consumed;
+ *   - rgb[e] and the three info slots keep their values; rew[e] = 0 and first[e] = 0, so that sums of rew and
+ *     counts of first over all envs stay correct;
+ *   - with final outputs, level_end[e] = 0 and the final rgb[e] keeps its value;
+ *   - with the consumer output, the ring moves on for every env (one ring position per handle): a paused env's
+ *     newest slot gets its current frame again, so its k-frame stack repeats the frame it is paused on (the older
+ *     frames are not zeroed: first = 0).
+ * Every env that is not paused steps exactly as on a handle without the mask, and an all-zero mask gives the
+ * outputs and states of a handle that never called this. Only the first kernel of a step reads the mask, so
+ * rewriting it while a step runs cannot split one env's step. Indices are the handle's own (env n of a joint
+ * list plays game n % G; local indices of a shard). get_state / set_state neither read nor write the mask;
+ * set_state into a paused env works as always, and the env stays paused.
+ * Ordering as for next_level_seed: with pgb200_act_device, write the mask on the handle's stream before the
+ * call; with libenv_act, the writes must be complete before the call. CUDA graphs: the first call is refused
+ * (-1) while the handle's stream captures; a captured step reads the mask only if it existed at capture, and
+ * then reads its contents at every replay. A handle without the mask runs the kernels it ran before. */
+LIBENV_API int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -222,13 +246,14 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * replay is the step issued at capture: same outputs as an eager call on the same inputs.
  * A captured step keeps what the host decided at capture: the launch shape (pgb200_set_launch_shape), the
  * level choice (the next_level_seed array is read only if pgb200_get_next_level_seeds had been called
- * before the capture), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
+ * before the capture; likewise the pause mask and pgb200_get_pause_mask), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
  * any of these afterwards leaves the graph as it was; capture again. Replays of one handle's graphs must be
  * ordered with each other and with its eager work (one stream, or events). pgb200_kernel_launches counts
  * launches issued, a captured step once, not its replays.
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
- * pgb200_get_next_level_seeds, pgb200_get_device_buffers before the initial reset, pgb200_set_consumer_output,
+ * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_get_device_buffers
+ * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
  * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step
  * cannot be captured with the peer mirror set (its parity is host state), with host buffers, or under

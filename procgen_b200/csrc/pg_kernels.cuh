@@ -61,6 +61,11 @@ struct KParams {
     uint8_t *level_end;         // [N] why env's level ended in this step (PGB200_LEVEL_END_*), 0 = it did not
     int32_t *reset_list;        // this launch's own segment of an [N] list: the envs phase B resets
     unsigned int *reset_count;  // entries in reset_list (device; beside the launch's ticket)
+    // optional pause mask (pgb200_get_pause_mask); null = off. Only the logic kernel reads the caller's array: it
+    // records each env's decision in `paused`, which the step's setup and render kernels read, so that every kernel
+    // of one step agrees even if the caller rewrites the mask while the step runs
+    const uint8_t *pause;       // [N] caller's mask: != 0 = env does not step
+    uint8_t *paused;            // [N] handle-owned: env is paused in the current step
 };
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
@@ -174,6 +179,22 @@ PG_HD void env_step_logic(const KParams &p, int env) {
     }
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, *c.h);
+}
+
+// The start of a step on a handle with a pause mask, before anything of the env is touched: records whether env is
+// paused in this step and, if it is, writes the outputs a paused step defines (rew = 0, first = 0, and level_end = 0
+// with final outputs). Its state, rgb and info slots keep their values. Returns whether env is paused.
+template <bool FINAL>
+PG_HD bool env_pause_logic(const KParams &p, int env) {
+    const uint8_t paused = p.pause[env] != 0;
+    p.paused[env] = paused;
+    if (paused) {
+        p.rew[env] = 0.f;
+        p.first[env] = 0;
+        if (FINAL)
+            p.level_end[env] = 0;
+    }
+    return paused != 0;
 }
 
 // Phase A of a step with final outputs: Game::step up to the reset decision, with the cause of a level end

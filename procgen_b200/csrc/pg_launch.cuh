@@ -70,7 +70,9 @@ constexpr int kRenderThreads = 128;
 // global ticket counter until the launch's range is exhausted, so a long env (level reset) only
 // delays its own warp and no SM slot idles waiting for a block launch.
 // FINAL: phase A of a step with final outputs; an env whose level ends is appended to p.reset_list.
-template <class G, bool INIT, bool LEVEL_CHOICE = false, bool FINAL = false>
+// PAUSE: the handle has a pause mask. A paused env's warp reads its entry, writes its outputs and takes the next
+// ticket without touching the env's state; it never enters phase B's list.
+template <class G, bool INIT, bool LEVEL_CHOICE = false, bool FINAL = false, bool PAUSE = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -85,7 +87,8 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
         const long long t0 = p.dbg_cycles ? clock64() : 0;
         if (INIT)
             env_init_logic<G, Frame>(p, env);
-        else if (FINAL) {
+        else if (PAUSE && env_pause_logic<FINAL>(p, env)) {
+        } else if (FINAL) {
             if (env_step_logic_final<G, Frame>(p, env) && lane == 0)
                 p.reset_list[atomicAdd(p.reset_count, 1u)] = env;
         } else
@@ -124,8 +127,9 @@ constexpr int kSetupThreads = 128;
 #ifndef PG_SETUP_MIN_BLOCKS
 #define PG_SETUP_MIN_BLOCKS 8   // 64 registers x 32 warps/SM: more envs in flight beat more registers (96 x 20 was slower)
 #endif
-// LIST: phase B of a step with final outputs, the warps of the grid stride over p.reset_list
-template <class G, int VIEW, bool LIST = false>
+// LIST: phase B of a step with final outputs, the warps of the grid stride over p.reset_list (which never holds a
+// paused env). PAUSE: a paused env's warp returns; its frame_setup slot goes stale, and nothing reads it.
+template <class G, int VIEW, bool LIST = false, bool PAUSE = false>
 __global__ void __launch_bounds__(kSetupThreads, PG_SETUP_MIN_BLOCKS) setup_kernel(KParams p) {
     using Setup = typename FrameFor<G, VIEW>::setup;
     const int i = (int)blockIdx.x * (kSetupThreads / 32) + (int)(threadIdx.x >> 5);
@@ -141,6 +145,8 @@ __global__ void __launch_bounds__(kSetupThreads, PG_SETUP_MIN_BLOCKS) setup_kern
     if (i >= p.env_count)
         return;
     const int env = p.env_first + i * p.env_step;
+    if (PAUSE && p.paused[env])
+        return;
     Setup &f = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
     env_setup_frame<G, Setup>(p, env, f, (int)(threadIdx.x & 31u), 32);
 }
@@ -305,16 +311,39 @@ __device__ __forceinline__ void render_env_frame(const KParams &p, typename Fram
 #undef PG_RENDER_PHASE
 }
 
+// A paused env's consumer epilogue. There is one ring position per handle, so the ring moves on for every env: the
+// newest slot s and its twin s + k get the frame the env is paused on, which is in slot s - 1 because every step
+// (and pgb200_set_consumer_output, and set_state) writes every env's current slot. Its older frames stay (first = 0).
+__device__ __forceinline__ void consumer_repeat_frame(const KParams &p, int env) {
+    constexpr int kSlotVecs = 3 * RES_W * RES_H * 2 / 16;  // 16-byte words of one 16-bit frame
+    const int kf = p.consumer_k, s = *p.consumer_slot_dev;
+    uint4 *base = reinterpret_cast<uint4 *>(p.consumer) + (size_t)env * (2 * kf) * kSlotVecs;
+    const uint4 *src = base + (size_t)((s - 1 + kf) % kf) * kSlotVecs;
+    for (int w = (int)threadIdx.x; w < kSlotVecs; w += kRenderThreads) {
+        const uint4 v = src[w];
+        base[(size_t)s * kSlotVecs + w] = v;
+        base[(size_t)(s + kf) * kSlotVecs + w] = v;
+    }
+}
+
 // PASS 0: a plain step, one CTA per env of the launch. With final outputs (pgb200_get_final_outputs):
 // PASS 1 (phase A), the same grid, but the frame of an env whose level ended is its final frame: it goes to
 // final_rgb and skips the consumer epilogue, whose episode-start rule would read the previous step's first[env].
 // PASS 2 (phase B), a fixed grid whose CTAs loop over the envs phase A listed, after their reset: the mbarrier is
 // re-armed per env with alternating parity, and the bulk store's wait_group.read 0 has already released the frame.
-template <class G, int VIEW, int PASS = 0>
+// PAUSE (PASS 0 and 1, a handle with a pause mask): the CTA of an env paused in this step renders nothing; its rgb
+// slot keeps the frame it is paused on, and the consumer ring gets that frame again (consumer_repeat_frame).
+template <class G, int VIEW, int PASS = 0, bool PAUSE = false>
 __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlocks) render_kernel(KParams p) {
+    static_assert(!(PAUSE && PASS == 2), "phase B's list never holds a paused env");
     using Frame = typename FrameFor<G, VIEW>::type;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Frame &f = *reinterpret_cast<Frame *>(smem_raw);
+    if (PAUSE && p.paused[p.env_first + (int)blockIdx.x * p.env_step]) {
+        if (p.consumer != nullptr && p.consumer_k > 1)
+            consumer_repeat_frame(p, p.env_first + (int)blockIdx.x * p.env_step);
+        return;
+    }
     if (threadIdx.x == 0)
         pg_mbar_init(&f.mbar, 1);
     __syncthreads();
@@ -383,7 +412,7 @@ struct LaunchCtx {
 #ifndef PG_HOSTSIM
 // Dynamic shared memory of one render CTA (frame, or the co-residency floor) with the kernel's
 // opt-in limit raised to it once.
-template <class G, int VIEW, int PASS = 0>
+template <class G, int VIEW, int PASS = 0, bool PAUSE = false>
 int prepare_render_smem(const LaunchCtx &lc) {
     using Frame = typename FrameFor<G, VIEW>::type;
     const int bytes = (int)sizeof(Frame) > lc.render_smem_floor ? (int)sizeof(Frame) : lc.render_smem_floor;
@@ -393,7 +422,7 @@ int prepare_render_smem(const LaunchCtx &lc) {
     CUDA_CHECK(cudaGetDevice(&dev));
     int &have = attr_set[dev & 63];
     if (have < bytes) {
-        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS, PAUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
         have = bytes;
     }
     return bytes;
@@ -407,26 +436,62 @@ int prepare_render_smem(const LaunchCtx &lc) {
 // ticket[0] is phase A's ticket, ticket[1] the list's count and ticket[2] phase B's ticket: one memset clears
 // all three. Phase B's grids are fixed (machine-filling) and read the count on the device, so nothing waits for
 // the host and the step stays capturable. Everything goes to lc.stream (a priority-split logic stream would
-// let the next launch that shares this ticket slot clear it under phase B).
-template <class G, int VIEW>
+// let the next launch that shares this ticket slot clear it under phase B). PAUSE: phase A skips paused envs, and
+// phase B, which only sees the list, needs no variant.
+template <class G, int VIEW, bool PAUSE>
 void launch_final_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
     KParams q = p;
     q.reset_count = lc.ticket + 1;
-    const int render_a = prepare_render_smem<G, VIEW, 1>(lc);
+    const int render_a = prepare_render_smem<G, VIEW, 1, PAUSE>(lc);
     const int render_b = prepare_render_smem<G, VIEW, 2>(lc);
     const int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
     const int setup_b = setup_blocks < lc.num_sms * PG_SETUP_MIN_BLOCKS ? setup_blocks : lc.num_sms * PG_SETUP_MIN_BLOCKS;
     const int render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
     const int render_blocks_b = p.env_count < render_fit ? p.env_count : render_fit;
     CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, 3 * sizeof(unsigned int), lc.stream));
-    logic_kernel<G, false, false, true><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
-    setup_kernel<G, VIEW><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(q);
-    render_kernel<G, VIEW, 1><<<p.env_count, kRenderThreads, render_a, lc.stream>>>(q);
+    logic_kernel<G, false, false, true, PAUSE><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
+    setup_kernel<G, VIEW, false, PAUSE><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(q);
+    render_kernel<G, VIEW, 1, PAUSE><<<p.env_count, kRenderThreads, render_a, lc.stream>>>(q);
     finish_kernel<G><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
     setup_kernel<G, VIEW, true><<<setup_b, kSetupThreads, 0, lc.stream>>>(q);
     render_kernel<G, VIEW, 2><<<render_blocks_b, kRenderThreads, render_b, lc.stream>>>(q);
     CUDA_CHECK(cudaGetLastError());
     (*lc.launch_counter) += 6;
+}
+#endif
+
+#ifndef PG_HOSTSIM
+// One (game, env chunk) launch of a plain step (or of the initial reset): logic, setup, render. PAUSE: the
+// instantiations that skip the envs the handle's pause mask holds still.
+template <class G, bool INIT, int VIEW, bool PAUSE>
+void launch_plain_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
+    // Shared memory per render CTA: the frame, or more when the handle asks for fewer resident
+    // render CTAs per SM. At 8 CTAs x 128 threads x 64 registers the render kernel owns the whole
+    // register file of an SM and no logic-kernel block of another env chunk can run beside it;
+    // capping its residency trades a little render speed for real overlap of the two kernels.
+    const int render_smem = prepare_render_smem<G, VIEW, 0, PAUSE>(lc);
+    cudaStream_t ls = lc.logic_stream ? lc.logic_stream : lc.stream;
+    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, sizeof(unsigned int), ls));
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[0], ls));
+    if (!INIT && p.next_level_seed)
+        logic_kernel<G, false, true, false, PAUSE><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
+    else
+        logic_kernel<G, INIT, false, false, PAUSE><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
+    if (lc.logic_stream) {
+        CUDA_CHECK(cudaEventRecord(lc.link, ls));
+        CUDA_CHECK(cudaStreamWaitEvent(lc.stream, lc.link, 0));
+    }
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
+    setup_kernel<G, VIEW, false, PAUSE><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
+    render_kernel<G, VIEW, 0, PAUSE><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
+    CUDA_CHECK(cudaGetLastError());
+    (*lc.launch_counter) += 3;
 }
 #endif
 
@@ -436,40 +501,22 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     if (p.env_count <= 0)
         return;
 #ifndef PG_HOSTSIM
-    // Shared memory per render CTA: the frame, or more when the handle asks for fewer resident
-    // render CTAs per SM. At 8 CTAs x 128 threads x 64 registers the render kernel owns the whole
-    // register file of an SM and no logic-kernel block of another env chunk can run beside it;
-    // capping its residency trades a little render speed for real overlap of the two kernels.
-    const int render_smem = prepare_render_smem<G, VIEW>(lc);
     int logic_blocks = (p.env_count + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
     if (logic_blocks > lc.max_logic_blocks)
         logic_blocks = lc.max_logic_blocks;
-    if (!INIT && p.level_end) {
-        launch_final_step<G, VIEW>(p, lc, logic_blocks);
-        return;
+    if constexpr (INIT) {
+        launch_plain_step<G, true, VIEW, false>(p, lc, logic_blocks);
+    } else {
+        // a handle without a pause mask runs exactly the kernels it ran before the mask existed
+        if (p.level_end && p.pause)
+            launch_final_step<G, VIEW, true>(p, lc, logic_blocks);
+        else if (p.level_end)
+            launch_final_step<G, VIEW, false>(p, lc, logic_blocks);
+        else if (p.pause)
+            launch_plain_step<G, false, VIEW, true>(p, lc, logic_blocks);
+        else
+            launch_plain_step<G, false, VIEW, false>(p, lc, logic_blocks);
     }
-    cudaStream_t ls = lc.logic_stream ? lc.logic_stream : lc.stream;
-    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, sizeof(unsigned int), ls));
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[0], ls));
-    if (!INIT && p.next_level_seed)
-        logic_kernel<G, false, true><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
-    else
-        logic_kernel<G, INIT><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
-    if (lc.logic_stream) {
-        CUDA_CHECK(cudaEventRecord(lc.link, ls));
-        CUDA_CHECK(cudaStreamWaitEvent(lc.stream, lc.link, 0));
-    }
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
-    setup_kernel<G, VIEW><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
-    render_kernel<G, VIEW><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
-    CUDA_CHECK(cudaGetLastError());
-    (*lc.launch_counter) += 3;
 #else
     static thread_local Frame *f = new Frame;
     if (!INIT && p.level_end) {
@@ -481,6 +528,8 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
         fin.rgb = p.final_rgb;
         for (int b = 0; b < p.env_count; b++) {
             const int env = p.env_first + b * p.env_step;
+            if (p.pause && env_pause_logic<true>(q, env))
+                continue;  // setup and render skip it (q.paused[env]), and it never enters the list
             const bool ended = env_step_logic_final<G, Frame>(q, env);
             if (ended)
                 q.reset_list[count++] = env;
@@ -497,6 +546,8 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
         int env = p.env_first + b * p.env_step;
         if (INIT)
             env_init_logic<G, Frame>(p, env);
+        else if (p.pause && env_pause_logic<false>(p, env))
+            continue;  // setup and render skip it (p.paused[env])
         else if (p.next_level_seed)
             env_step_logic<G, Frame, true>(p, env);
         else

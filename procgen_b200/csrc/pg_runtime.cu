@@ -243,6 +243,9 @@ struct VecEnv {
     int32_t *d_next_level_seed = nullptr;   // allocated by the first pgb200_get_next_level_seeds
     // allocated by the first pgb200_get_final_outputs: base.final_rgb, base.level_end and the pending-reset list
     int32_t *d_reset_list = nullptr;
+    // allocated by the first pgb200_get_pause_mask: the caller's mask (base.pause) and what the logic kernel
+    // recorded of it for the step's later kernels (base.paused)
+    uint8_t *d_pause = nullptr, *d_paused = nullptr;
     bool initial_reset_done = false;
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
@@ -991,6 +994,8 @@ void libenv_close(libenv_env *handle) {
     dev_free(p.final_rgb);
     dev_free(p.level_end);
     dev_free(v->d_reset_list);
+    dev_free(v->d_pause);
+    dev_free(v->d_paused);
     dev_free(p.rgb);
     dev_free(p.rew);
     dev_free(p.first);
@@ -1114,6 +1119,32 @@ int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *ou
     }
     out->rgb = v->base.final_rgb;
     out->level_end = v->base.level_end;
+    return 0;
+}
+
+int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    if ((!v->initial_reset_done || !v->d_pause) && v->capturing())
+        return -1;
+    v->ensure_initial_reset();
+    if (!v->d_pause) {
+        const size_t N = (size_t)v->num_envs ? (size_t)v->num_envs : 1;
+#ifndef PG_HOSTSIM
+        CUDA_CHECK(cudaMalloc((void **)&v->d_pause, N));
+        CUDA_CHECK(cudaMalloc((void **)&v->d_paused, N));
+        CUDA_CHECK(cudaMemsetAsync(v->d_pause, 0, N, v->stream));
+        CUDA_CHECK(cudaMemsetAsync(v->d_paused, 0, N, v->stream));
+        // complete before the caller writes, from whatever stream it writes on
+        v->sync();
+#else
+        v->d_pause = (uint8_t *)calloc(N, 1);
+        v->d_paused = (uint8_t *)calloc(N, 1);
+#endif
+        v->base.pause = v->d_pause;
+        v->base.paused = v->d_paused;
+    }
+    *out = v->d_pause;
     return 0;
 }
 

@@ -137,6 +137,7 @@ class BaseProcgenEnv:
         self._torch = None
         self._next_level_seeds = None
         self._final_outputs = None
+        self._pause_mask = None
         self._consumer_slot = None
         self._graph_stepped = False   # act() has run inside a CUDA graph capture
         self._retired_consumers = []  # consumer buffers a captured graph may still write
@@ -270,8 +271,9 @@ class BaseProcgenEnv:
         Inside ``torch.cuda.graph`` (or any capture on the current stream) act() takes a CUDA tensor only and
         the step becomes part of the graph: the handle is rebound to the capture stream without a host wait,
         and every replay steps the envs again with whatever the action tensor then holds. Set up before the
-        capture what the step should use (next_level_seeds(), enable_consumer_output(), set_launch_shape()):
-        a graph keeps the launch shape, the level choice and the consumer output it was captured with."""
+        capture what the step should use (next_level_seeds(), pause_mask(), enable_consumer_output(),
+        set_launch_shape()): a graph keeps the launch shape, the level choice, the pause mask and the consumer output
+        it was captured with."""
         if self._capturing():
             if self._host_buffers:
                 raise RuntimeError("procgen_b200: act() cannot be captured in a CUDA graph with host_buffers=True; "
@@ -287,10 +289,12 @@ class BaseProcgenEnv:
             self._graph_stepped = True
         if self._host_buffers:
             self._ac[:] = np.asarray(ac).astype(np.int32)
-            if self._next_level_seeds is not None:
-                # libenv_act reads the level choices on the library's own stream: the caller's torch writes
-                # must be complete first
-                self._torch.cuda.current_stream(self._next_level_seeds.device).synchronize()
+            for arr in (self._next_level_seeds, self._pause_mask):
+                if arr is not None:
+                    # libenv_act reads the level choices and the pause mask on the library's own stream: the
+                    # caller's torch writes must be complete first
+                    self._torch.cuda.current_stream(arr.device).synchronize()
+                    break
             self._lib.libenv_act(self._h)
             return
         torch = self._torch
@@ -390,6 +394,32 @@ class BaseProcgenEnv:
                     "level_end": torch.as_tensor(_CudaArray(out.level_end, (self.num,), "|u1"), device=dev),
                 }
         return dict(self._final_outputs)
+
+    def pause_mask(self):
+        """uint8 CUDA tensor [num] aliasing the library's per-env pause mask (allocated, all 0, on the first call). In
+        every step, env e with mask[e] != 0 is paused: its state stays as it is, byte for byte (a paused step does
+        not count toward the time limit), its action (-1 included) is ignored and its next_level_seeds() entry is
+        neither read nor consumed; its rgb and info slots keep their values, and rew[e] = 0, first[e] = 0 (and
+        final_outputs()["level_end"][e] = 0). With the consumer output on, the stack of a paused env repeats the
+        frame it is paused on. Every other env steps exactly as it would without the mask. A step does not clear
+        the mask: an entry stays in force until the caller clears it. get_state / set_state neither read nor
+        change it.
+
+        Write it with torch ops on the stream you step on (device-resident mode); with host_buffers=True, act()
+        waits for the current torch stream before it starts the step.
+
+        A CUDA graph reads the mask only if it was requested before the capture: call this once first. Inside the
+        capture the tensor may then be refilled with torch ops like any other input of the graph."""
+        if self._pause_mask is None:
+            self._refuse_in_capture("pause_mask")
+            torch = self._torch
+            ptr = C.POINTER(C.c_uint8)()
+            with torch.cuda.device(self.device_index):
+                if self._lib.pgb200_get_pause_mask(self._h, C.byref(ptr)) != 0:
+                    raise RuntimeError("pgb200_get_pause_mask failed")
+                dev = torch.device("cuda", self.device_index)
+                self._pause_mask = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "|u1"), device=dev)
+        return self._pause_mask
 
     def callmethod(self, method: str, *args, **kwargs):
         return getattr(self, method)(*args, **kwargs)
@@ -615,6 +645,7 @@ class BaseProcgenEnv:
         if getattr(self, "_h", None):
             self._next_level_seeds = None
             self._final_outputs = None
+            self._pause_mask = None
             self._lib.libenv_close(self._h)
             self._h = None
 
