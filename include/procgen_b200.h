@@ -228,6 +228,32 @@ LIBENV_API int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_
  * then reads its contents at every replay. A handle without the mask runs the kernels it ran before. */
 LIBENV_API int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out);
 
+/* Level bank: levels generated once and copied in at reset. A generated level is a pure function of the game, the
+ * options and the seed, so a handle that keeps resetting onto the same few hundred seeds (num_levels = 200 or
+ * 500, a held-out seed list, a level-replay buffer) can keep them instead of generating them again.
+ * pgb200_build_level_bank banks `seeds[0, count)` (host memory; every seed in [0, 2^31); duplicates are allowed)
+ * for every game of the handle's list. The first call allocates room for max(count, capacity) distinct seeds per
+ * game; that capacity is then fixed. A later call rebuilds the bank in place, on the handle's stream and ordered
+ * with its steps, so graphs captured earlier stay valid and see the new bank. count == 0 empties it. Performs the
+ * initial reset if it has not happened yet, and returns when the bank is built. Returns 0, or -1 (nothing changed)
+ * when a seed is out of range, there are more distinct seeds than the capacity, a first call has
+ * max(count, capacity) == 0 (a bank that could never hold a level), or the handle's stream is capturing (the call
+ * allocates and waits). Slots are sized per game of the list; a level that needs more entities or cells than its
+ * game's capacities (possible only in a joint list) is generated at every reset instead.
+ * At every reset inside a step, the new level's seed s is chosen as always (game end, time limit, action -1, a
+ * next_level_seed override, the +997 of sequential levels). If s is banked and the env's options are the ones the
+ * bank was generated with (all but center_agent, which level generation only writes; an env can differ only
+ * after set_state of a blob made under other options), the reset copies the banked level instead of generating
+ * it. Every output and every state byte is identical to a handle without a bank: its only effect is speed.
+ * The initial reset, get_state / set_state, the wire format and next_level_seed consumption are unaffected; a
+ * paused env never resets; phase B of final outputs uses the bank like any other reset.
+ * CUDA graphs: a captured step uses the bank if one existed at capture, and a rebuild is seen by later replays;
+ * a step captured without a bank never uses one. A handle without a bank runs the kernels it ran before.
+ * pgb200_level_bank_info: *levels = the distinct seeds banked now, *bytes = the device memory the bank holds
+ * (0 and 0 without one). Returns 0. */
+LIBENV_API int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count, int capacity);
+LIBENV_API int pgb200_level_bank_info(libenv_env *handle, int *levels, int64_t *bytes);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -252,7 +278,7 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * launches issued, a captured step once, not its replays.
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
- * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_get_device_buffers
+ * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank, pgb200_get_device_buffers
  * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
  * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step

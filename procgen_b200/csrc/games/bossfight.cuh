@@ -19,6 +19,9 @@ struct BossfightGame : Defaults<BossfightGame>, DrawDefaults<BossfightGame> {
     static constexpr int ENT_CAP = 384;
     static constexpr int GRID_CAP = 20 * 20;
     static constexpr int SCRATCH_WORDS = 0;
+    // rand_pct, rand_fire_pct, rand_pct_x, rand_pct_y: drawn at the start of every step, never by game_reset
+    static constexpr int STEP_STATE_OFFSET = (int)offsetof(BossfightState, rand_pct);
+    static constexpr int STEP_STATE_BYTES = 4 * (int)sizeof(float);
     static constexpr int MAX_VISIBLE_ENTS = 384;
     static constexpr int MAX_ROT_BLITS = 352;  // every enemy bullet and its trails spin (vrot = PI/8)
     static constexpr int MAX_VIEW_CELLS = 20;

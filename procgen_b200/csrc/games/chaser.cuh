@@ -17,6 +17,8 @@ struct ChaserGame : Defaults<ChaserGame>, DrawDefaults<ChaserGame> {
     static constexpr int MAZE_WORDS = 4800;       // MazeGen::words_needed(19) = 4721
     static constexpr int LIST_WORDS = 400;
     static constexpr int SCRATCH_WORDS = MAZE_WORDS + 4 * LIST_WORDS;
+    static constexpr int PERSIST_SCRATCH_FIRST = MAZE_WORDS;  // free_cells and is_space_vec; the maze and the quadrant lists are workspace
+    static constexpr int PERSIST_SCRATCH_WORDS = 2 * LIST_WORDS;
     static constexpr int MAX_VISIBLE_ENTS = 64;
     static constexpr int MAX_ROT_BLITS = 0;
     static constexpr int MAX_VIEW_CELLS = 19;

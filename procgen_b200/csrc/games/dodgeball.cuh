@@ -16,6 +16,8 @@ struct DodgeballGame : Defaults<DodgeballGame>, DrawDefaults<DodgeballGame> {
     static constexpr int GRID_CAP = 40 * 40;
     static constexpr int MAX_ROOMS = 64;  // <= 1 + 2 * 16 splits
     static constexpr int SCRATCH_WORDS = 4 * MAX_ROOMS;
+    static constexpr int PERSIST_SCRATCH_FIRST = 0;  // the room list
+    static constexpr int PERSIST_SCRATCH_WORDS = SCRATCH_WORDS;
     static constexpr int MAX_VISIBLE_ENTS = 256;  // lava walls are tiled; only the on-screen run of tiles becomes blits (measured peak 119)
     static constexpr int MAX_ROT_BLITS = 64;      // everything that faces a direction or spins (measured peak 20)
     static constexpr int MAX_VIEW_CELLS = 20;

@@ -13,6 +13,9 @@ struct MinerGame : Defaults<MinerGame>, DrawDefaults<MinerGame> {
     static constexpr int ENT_CAP = 16;
     static constexpr int GRID_CAP = 35 * 35;
     static constexpr int SCRATCH_WORDS = 4 * 1280;
+    // diamonds_remaining: counted by every step, never by game_reset
+    static constexpr int STEP_STATE_OFFSET = (int)offsetof(MinerState, diamonds_remaining);
+    static constexpr int STEP_STATE_BYTES = (int)sizeof(int32_t);
     static constexpr int MAX_VISIBLE_ENTS = 64;
     static constexpr int MAX_ROT_BLITS = 0;
     static constexpr bool ENTS_BELOW_GRID = true;  // the exit sits under the grid layer (render_z = -1, miner.cpp:199)

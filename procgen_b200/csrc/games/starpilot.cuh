@@ -21,6 +21,8 @@ struct StarpilotGame : Defaults<StarpilotGame>, DrawDefaults<StarpilotGame> {
     static constexpr int MAX_SPAWNERS = 256;
     static constexpr int ENT_WORDS = (int)(sizeof(Entity) / 4);
     static constexpr int SCRATCH_WORDS = MAX_SPAWNERS * ENT_WORDS + MAX_SPAWNERS;
+    static constexpr int PERSIST_SCRATCH_FIRST = 0;  // the spawner list
+    static constexpr int PERSIST_SCRATCH_WORDS = SCRATCH_WORDS;
     static constexpr int MAX_VISIBLE_ENTS = 256;
     static constexpr int MAX_ROT_BLITS = 224;  // ships, bullets and the agent all carry a rotation
     static constexpr int MAX_VIEW_CELLS = 16;

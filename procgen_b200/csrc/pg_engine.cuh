@@ -12,7 +12,7 @@
 // Expression types (float vs double, int promotion) are kept exactly as in the reference line
 // each function cites, because results must be bit-identical; see pg_common.cuh.
 #pragma once
-#include "pg_state.cuh"
+#include "pg_bank.cuh"
 
 namespace pg {
 
@@ -789,7 +789,9 @@ struct Engine {
     // ---- Game::reset / Game::step (game.cpp:93-155)
     // level_seed_override >= 0 (pgb200_get_next_level_seeds) replaces the draw of the next level seed and
     // nothing else: level_seed_rand_gen is not advanced. Returns whether the override was taken.
-    static PG_HD bool reset(Ctx &c, int32_t level_seed_override = -1) {
+    // BANK: a level the bank holds (bank_copy_level) is copied instead of generated; nothing else changes.
+    template <bool BANK = false>
+    static PG_HD bool reset(Ctx &c, int32_t level_seed_override = -1, const LevelBank *bank = nullptr) {
         EnvHdr &h = *c.h;
         bool took = false;
         h.reset_count++;
@@ -808,8 +810,10 @@ struct Engine {
             h.done = 0;
             h.level_complete = 0;
         }
-        mt_seed(*c.rng, (uint32_t)h.current_level_seed);
-        G::game_reset(c);
+        if (!BANK || !bank_copy_level<G>(c, *bank)) {
+            mt_seed(*c.rng, (uint32_t)h.current_level_seed);
+            G::game_reset(c);
+        }
         h.cur_time = 0;
         h.total_reward = 0;
         h.episodes_remaining -= 1;
@@ -847,11 +851,12 @@ struct Engine {
         h.prev_level_seed = h.current_level_seed;
         return h.done != 0;
     }
-    static PG_HD bool step_finish(Ctx &c, bool do_reset, int32_t level_seed_override) {
+    template <bool BANK = false>
+    static PG_HD bool step_finish(Ctx &c, bool do_reset, int32_t level_seed_override, const LevelBank *bank = nullptr) {
         EnvHdr &h = *c.h;
         bool took = false;
         if (do_reset)
-            took = reset(c, level_seed_override);
+            took = reset<BANK>(c, level_seed_override, bank);
         if (h.options.use_sequential_levels && h.level_complete)
             h.done = 0;
         h.episode_done = h.done;
@@ -953,6 +958,14 @@ struct Defaults {
     static PG_HD void update_agent_velocity(Ctx &c) { E::default_update_agent_velocity(c); }
     static PG_HD void game_step(Ctx &c) { E::basic_game_step(c); }
     static PG_HD void game_reset(Ctx &c) { E::basic_game_reset(c); }
+    // scratch words [PERSIST_SCRATCH_FIRST, + PERSIST_SCRATCH_WORDS) outlive game_reset (the game's steps or its
+    // state blob read them); every other scratch word is level-generation workspace. A banked level carries these.
+    static constexpr int PERSIST_SCRATCH_FIRST = 0;
+    static constexpr int PERSIST_SCRATCH_WORDS = 0;
+    // bytes [STEP_STATE_OFFSET, + STEP_STATE_BYTES) of the game's state struct (game_state) are written by its steps
+    // and never by game_reset, so that a reset inherits them from the episode before; a banked level leaves them be
+    static constexpr int STEP_STATE_OFFSET = 0;
+    static constexpr int STEP_STATE_BYTES = 0;
     // bookkeeping hooks for games that hold references to entities (shared_ptr members); a game
     // that defines them sets HAS_ENTITY_HOOKS
     static constexpr bool HAS_ENTITY_HOOKS = false;

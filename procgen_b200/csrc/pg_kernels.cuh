@@ -66,6 +66,10 @@ struct KParams {
     // of one step agrees even if the caller rewrites the mask while the step runs
     const uint8_t *pause;       // [N] caller's mask: != 0 = env does not step
     uint8_t *paused;            // [N] handle-owned: env is paused in the current step
+    // optional level bank (pgb200_build_level_bank); bank.slots null = off. The launch's game's slots. A banked
+    // handle steps in two phases as with final outputs; without them, phase A's level_end goes to bank_level_end
+    LevelBank bank;
+    uint8_t *bank_level_end;    // [N] handle-owned
 };
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
@@ -221,14 +225,72 @@ PG_HD bool env_step_logic_final(const KParams &p, int env) {
 
 // Phase B: the rest of Game::step for an env whose level ended in phase A. The reset reads and consumes the
 // env's next_level_seed entry as env_step_logic<LEVEL_CHOICE> does; then Game::observe's camera and scalars.
-template <class G, class Frame>
+// BANK: the handle has a level bank, which the reset copies the level from when it holds it.
+template <class G, class Frame, bool BANK = false>
 PG_HD void env_finish_logic(const KParams &p, int env) {
     Ctx c = make_ctx(p, env);
     const int32_t next_seed = p.next_level_seed ? p.next_level_seed[env] : -1;
-    if (Engine<G>::step_finish(c, true, next_seed))
+    if (Engine<G>::template step_finish<BANK>(c, true, next_seed, &p.bank))
         p.next_level_seed[env] = -1;
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, *c.h);
+}
+
+// Level bank build: per-warp staging, the env's own record at the handle's capacities (EnvHdr, entities, grid,
+// rand_gen, level-generation scratch), 16-byte aligned parts
+PG_HD size_t bank_stage_bytes(const KParams &p) {
+    return sizeof(EnvHdr) + (size_t)p.ent_stride * sizeof(Entity) + (((size_t)p.grid_stride * sizeof(int16_t) + 15) & ~(size_t)15) +
+           sizeof(MT19937) + (((size_t)p.scratch_stride * sizeof(int32_t) + 15) & ~(size_t)15);
+}
+
+// Generates the level of bank.seeds[item] of the launch's game in `stage`, as a reset would from the state
+// init_constants leaves with the handle's options, then stores it in slot `item`, marked usable if it fits the
+// game's slot. One warp (or one thread in the host debug build).
+template <class G>
+PG_HD void bank_generate_level(const KParams &p, int item, unsigned char *stage) {
+    const LevelBank &b = p.bank;
+    Ctx c;
+    c.h = reinterpret_cast<EnvHdr *>(stage);
+    c.ents = reinterpret_cast<Entity *>(stage + sizeof(EnvHdr));
+    c.grid = reinterpret_cast<int16_t *>(stage + sizeof(EnvHdr) + (size_t)p.ent_stride * sizeof(Entity));
+    c.rng = reinterpret_cast<MT19937 *>(reinterpret_cast<unsigned char *>(c.grid) + (((size_t)p.grid_stride * sizeof(int16_t) + 15) & ~(size_t)15));
+    c.scratch = reinterpret_cast<int32_t *>(c.rng + 1);
+    c.lvl_rng = nullptr;  // game_reset never draws a level seed
+    c.assets = p.assets;
+    c.ent_cap = p.ent_stride - 1;
+    c.grid_cap = p.grid_stride;
+    c.scratch_cap = p.scratch_stride;
+    c.obst_hi = -1;
+    c.rot_scratch_raw = nullptr;
+    c.blit_list = nullptr;
+    c.cell_spill = nullptr;
+    G::init_constants(c);
+    EnvHdr &h = *c.h;
+    h.options = p.options;
+    h.options.center_agent = BANK_CENTER_AGENT_UNSET;
+    h.game_id = p.game_id;
+    h.fixed_asset_seed = p.fixed_asset_seed;
+    h.level_seed_low = p.level_seed_low;
+    h.level_seed_high = p.level_seed_high;
+    h.current_level_seed = b.seeds[item];
+    h.episodes_remaining = 1;
+    ctx_refresh(c);
+    mt_seed(*c.rng, (uint32_t)h.current_level_seed);
+    G::game_reset(c);
+    unsigned char *slot = b.slots + (size_t)item * b.slot_bytes;
+    const bool usable = h.max_ents_seen <= G::ENT_CAP && h.grid_size <= G::GRID_CAP && h.agent_idx < c.ent_cap;
+    if (usable) {
+        bank_copy_vecs(slot + BANK_SLOT_HEAD, &h, (int)sizeof(EnvHdr));
+        bank_copy_vecs(slot + b.ents_off, c.ents, h.n_ents * (int)sizeof(Entity));
+        int16_t *dg = reinterpret_cast<int16_t *>(slot + b.grid_off);
+        const int16_t *sg = c.grid;
+        pg_warp_for(h.grid_size, [=](int k) { dg[k] = sg[k]; });
+        bank_copy_vecs(slot + b.rng_off, c.rng, (int)sizeof(MT19937));
+        int32_t *ds = reinterpret_cast<int32_t *>(slot + b.scratch_off);
+        const int32_t *ss = c.scratch + G::PERSIST_SCRATCH_FIRST;
+        pg_warp_for(G::PERSIST_SCRATCH_WORDS, [=](int k) { ds[k] = ss[k]; });
+    }
+    *reinterpret_cast<int32_t *>(slot) = usable ? 1 : 0;  // every lane stores the same value
 }
 
 // ---- setup kernel body: one warp (lanes `lane` of `nlanes`) prepares everything about env's frame that

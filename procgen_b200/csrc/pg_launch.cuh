@@ -101,7 +101,8 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
 
 // Phase B of a step with final outputs: the resets of the envs phase A listed. Persistent and ticketed like the
 // logic kernel, because level generation runs here (milliseconds for caveflyer, jumper and leaper).
-template <class G>
+// BANK: the handle has a level bank; the only kernel a banked step adds to those of an unbanked one.
+template <class G, bool BANK = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -113,7 +114,25 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_ker
         t = __shfl_sync(0xffffffffu, t, 0);
         if (t >= count)
             break;
-        env_finish_logic<G, Frame>(p, p.reset_list[t]);
+        const int env = p.reset_list[t];
+        // a banked step's reset runs here: its cycles join phase A's in the profiling aid
+        const long long t0 = (BANK && p.dbg_cycles) ? clock64() : 0;
+        env_finish_logic<G, Frame, BANK>(p, env);
+        __syncwarp();
+        if (BANK && p.dbg_cycles && lane == 0)
+            p.dbg_cycles[env] += (uint32_t)(clock64() - t0);
+    }
+}
+
+// Level bank build: warp w generates the levels w, w + warps, ... of p.bank into their slots, in the staging area
+// stage + w * bank_stage_bytes(p) (the bank's memory budget bounds how many warps run)
+template <class G>
+__global__ void __launch_bounds__(kLogicThreads) bank_build_kernel(KParams p, unsigned char *stage, int count, int warps) {
+    const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (w >= warps)
+        return;
+    for (int item = w; item < count; item += warps) {
+        bank_generate_level<G>(p, item, stage + (size_t)w * bank_stage_bytes(p));
         __syncwarp();
     }
 }
@@ -438,7 +457,7 @@ int prepare_render_smem(const LaunchCtx &lc) {
 // the host and the step stays capturable. Everything goes to lc.stream (a priority-split logic stream would
 // let the next launch that shares this ticket slot clear it under phase B). PAUSE: phase A skips paused envs, and
 // phase B, which only sees the list, needs no variant.
-template <class G, int VIEW, bool PAUSE>
+template <class G, int VIEW, bool PAUSE, bool BANK>
 void launch_final_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
     KParams q = p;
     q.reset_count = lc.ticket + 1;
@@ -452,11 +471,41 @@ void launch_final_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) 
     logic_kernel<G, false, false, true, PAUSE><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
     setup_kernel<G, VIEW, false, PAUSE><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(q);
     render_kernel<G, VIEW, 1, PAUSE><<<p.env_count, kRenderThreads, render_a, lc.stream>>>(q);
-    finish_kernel<G><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
+    finish_kernel<G, BANK><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
     setup_kernel<G, VIEW, true><<<setup_b, kSetupThreads, 0, lc.stream>>>(q);
     render_kernel<G, VIEW, 2><<<render_blocks_b, kRenderThreads, render_b, lc.stream>>>(q);
     CUDA_CHECK(cudaGetLastError());
     (*lc.launch_counter) += 6;
+}
+#endif
+
+#ifndef PG_HOSTSIM
+// One (game, env chunk) launch of a plain step on a handle with a level bank and without final outputs. Its resets
+// run in a kernel of their own, so that the step itself runs the logic kernel it always runs (its stack frame and
+// registers stay those of the step, which must fit the push_obj / sub_step recursion): phase A of a step with final
+// outputs (level_end to the handle's own bank_level_end), the finish kernel over its list, where the resets copy
+// their levels from the bank, then one setup and one render over the launch's envs. Tickets as launch_final_step.
+template <class G, int VIEW, bool PAUSE>
+void launch_banked_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
+    KParams q = p;
+    q.level_end = p.bank_level_end;
+    q.reset_count = lc.ticket + 1;
+    const int render_smem = prepare_render_smem<G, VIEW, 0, PAUSE>(lc);
+    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, 3 * sizeof(unsigned int), lc.stream));
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[0], lc.stream));
+    logic_kernel<G, false, false, true, PAUSE><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
+    finish_kernel<G, true><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
+    setup_kernel<G, VIEW, false, PAUSE><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
+    render_kernel<G, VIEW, 0, PAUSE><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
+    if (lc.tev)
+        CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
+    CUDA_CHECK(cudaGetLastError());
+    (*lc.launch_counter) += 4;
 }
 #endif
 
@@ -506,12 +555,21 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
         logic_blocks = lc.max_logic_blocks;
     if constexpr (INIT) {
         launch_plain_step<G, true, VIEW, false>(p, lc, logic_blocks);
-    } else {
-        // a handle without a pause mask runs exactly the kernels it ran before the mask existed
+    } else if (p.bank.slots) {
         if (p.level_end && p.pause)
-            launch_final_step<G, VIEW, true>(p, lc, logic_blocks);
+            launch_final_step<G, VIEW, true, true>(p, lc, logic_blocks);
         else if (p.level_end)
-            launch_final_step<G, VIEW, false>(p, lc, logic_blocks);
+            launch_final_step<G, VIEW, false, true>(p, lc, logic_blocks);
+        else if (p.pause)
+            launch_banked_step<G, VIEW, true>(p, lc, logic_blocks);
+        else
+            launch_banked_step<G, VIEW, false>(p, lc, logic_blocks);
+    } else {
+        // a handle without a pause mask or a level bank runs exactly the kernels it ran before they existed
+        if (p.level_end && p.pause)
+            launch_final_step<G, VIEW, true, false>(p, lc, logic_blocks);
+        else if (p.level_end)
+            launch_final_step<G, VIEW, false, false>(p, lc, logic_blocks);
         else if (p.pause)
             launch_plain_step<G, false, VIEW, true>(p, lc, logic_blocks);
         else
@@ -519,6 +577,28 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     }
 #else
     static thread_local Frame *f = new Frame;
+    if (!INIT && !p.level_end && p.bank.slots) {
+        // the serial twin of launch_banked_step
+        unsigned int count = 0;
+        KParams q = p;
+        q.level_end = p.bank_level_end;
+        q.reset_count = &count;
+        for (int b = 0; b < p.env_count; b++) {
+            const int env = p.env_first + b * p.env_step;
+            if (p.pause && env_pause_logic<true>(q, env))
+                continue;
+            if (env_step_logic_final<G, Frame>(q, env))
+                q.reset_list[count++] = env;
+        }
+        for (unsigned int j = 0; j < count; j++) env_finish_logic<G, Frame, true>(q, q.reset_list[j]);
+        for (int b = 0; b < p.env_count; b++) {
+            const int env = p.env_first + b * p.env_step;
+            if (!(p.pause && p.paused[env]))
+                render_env_serial<G, VIEW, Frame>(p, env, *f);
+        }
+        (*lc.launch_counter) += 4;
+        return;
+    }
     if (!INIT && p.level_end) {
         // the serial twin of launch_final_step's two phases
         unsigned int count = 0;
@@ -536,7 +616,10 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
             render_env_serial<G, VIEW, Frame>(ended ? fin : q, env, *f);
         }
         for (unsigned int j = 0; j < count; j++) {
-            env_finish_logic<G, Frame>(q, q.reset_list[j]);
+            if (p.bank.slots)
+                env_finish_logic<G, Frame, true>(q, q.reset_list[j]);
+            else
+                env_finish_logic<G, Frame>(q, q.reset_list[j]);
             render_env_serial<G, VIEW, Frame>(q, q.reset_list[j], *f);
         }
         (*lc.launch_counter) += 6;
@@ -582,6 +665,23 @@ void launch_observe_only(const KParams &p, const LaunchCtx &lc) {
     (*lc.launch_counter) += 2;
 }
 
+// Generates p.bank's levels [0, count) of the launch's game: `warps` warps, each with bank_stage_bytes(p) of `stage`
+template <class G>
+void launch_bank_build(const KParams &p, const LaunchCtx &lc, unsigned char *stage, int warps, int count) {
+    if (count <= 0)
+        return;
+#ifndef PG_HOSTSIM
+    const int blocks = (warps + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
+    bank_build_kernel<G><<<blocks, kLogicThreads, 0, lc.stream>>>(p, stage, count, warps);
+    CUDA_CHECK(cudaGetLastError());
+    (*lc.launch_counter) += 1;
+#else
+    (void)lc;
+    (void)warps;
+    for (int item = 0; item < count; item++) bank_generate_level<G>(p, item, stage);
+#endif
+}
+
 struct GameVTable {
     const char *name;
     int id;
@@ -596,6 +696,8 @@ struct GameVTable {
     void (*init[2])(const KParams &, const LaunchCtx &);
     void (*step[2])(const KParams &, const LaunchCtx &);
     void (*observe_only[2])(const KParams &, const LaunchCtx &);
+    void (*bank_build)(const KParams &, const LaunchCtx &, unsigned char *, int, int);
+    int persist_scratch_words;  // G::PERSIST_SCRATCH_WORDS
 };
 
 template <class G, int VIEW>
@@ -622,6 +724,8 @@ GameVTable make_vtable(int id) {
     vt.ent_cap = G::ENT_CAP;
     vt.grid_cap = G::GRID_CAP;
     vt.scratch_words = G::SCRATCH_WORDS;
+    vt.persist_scratch_words = G::PERSIST_SCRATCH_WORDS;
+    vt.bank_build = &launch_bank_build<G>;
     vt.rot_records = FrameFor<G>::type::kMaxRot;
     vt.blit_records = FrameFor<G>::type::kMaxList;
     fill_view<G, G::MAX_VIEW_CELLS>(vt, 0);

@@ -13,6 +13,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <random>
 #include <stdexcept>
 #include <string>
@@ -246,6 +247,13 @@ struct VecEnv {
     // allocated by the first pgb200_get_pause_mask: the caller's mask (base.pause) and what the logic kernel
     // recorded of it for the step's later kernels (base.paused)
     uint8_t *d_pause = nullptr, *d_paused = nullptr;
+    // allocated by the first pgb200_build_level_bank: bank_capacity slots per game of the list, sized by the game
+    // (banks[g], one allocation at base.bank.slots), the sorted seed list they share and its length on the device
+    std::vector<LevelBank> banks;
+    int32_t *d_bank_seeds = nullptr, *d_bank_count = nullptr;
+    int bank_capacity = 0;
+    int bank_levels = 0;
+    int64_t bank_bytes = 0;
     bool initial_reset_done = false;
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
@@ -370,6 +378,8 @@ struct VecEnv {
                 p.env_count = hi - lo;
                 if (base.reset_list)
                     p.reset_list = base.reset_list + g * per_game + lo;  // the launch's own segment
+                if (base.bank.slots)
+                    p.bank = banks[g];
                 LaunchCtx lc = lctx();
 #ifndef PG_HOSTSIM
                 if (nstreams) {
@@ -996,6 +1006,10 @@ void libenv_close(libenv_env *handle) {
     dev_free(v->d_reset_list);
     dev_free(v->d_pause);
     dev_free(v->d_paused);
+    dev_free(p.bank.slots);
+    dev_free(p.bank_level_end);
+    dev_free(v->d_bank_seeds);
+    dev_free(v->d_bank_count);
     dev_free(p.rgb);
     dev_free(p.rew);
     dev_free(p.first);
@@ -1105,7 +1119,8 @@ int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *ou
 #ifndef PG_HOSTSIM
         CUDA_CHECK(cudaMalloc((void **)&v->base.final_rgb, frames));
         CUDA_CHECK(cudaMalloc((void **)&v->base.level_end, N));
-        CUDA_CHECK(cudaMalloc((void **)&v->d_reset_list, N * sizeof(int32_t)));
+        if (!v->d_reset_list)  // a level bank may have allocated it
+            CUDA_CHECK(cudaMalloc((void **)&v->d_reset_list, N * sizeof(int32_t)));
         CUDA_CHECK(cudaMemsetAsync(v->base.final_rgb, 0, frames, v->stream));
         CUDA_CHECK(cudaMemsetAsync(v->base.level_end, 0, N, v->stream));
         // complete before the caller reads, from whatever stream it reads on
@@ -1113,7 +1128,8 @@ int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *ou
 #else
         v->base.final_rgb = (uint8_t *)calloc(frames, 1);
         v->base.level_end = (uint8_t *)calloc(N, 1);
-        v->d_reset_list = (int32_t *)calloc(N, sizeof(int32_t));
+        if (!v->d_reset_list)
+            v->d_reset_list = (int32_t *)calloc(N, sizeof(int32_t));
 #endif
         v->base.reset_list = v->d_reset_list;
     }
@@ -1145,6 +1161,105 @@ int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
         v->base.paused = v->d_paused;
     }
     *out = v->d_pause;
+    return 0;
+}
+
+int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count, int capacity) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    if (count < 0 || capacity < 0 || (count > 0 && !seeds))
+        return -1;
+    for (int i = 0; i < count; i++)
+        if (seeds[i] < 0)
+            return -1;
+    if (v->capturing())
+        return -1;
+    std::vector<int32_t> sorted(seeds, seeds + count);
+    std::sort(sorted.begin(), sorted.end());
+    sorted.erase(std::unique(sorted.begin(), sorted.end()), sorted.end());
+    const int n = (int)sorted.size();
+    if (v->base.bank.slots ? n > v->bank_capacity : std::max(count, capacity) == 0)
+        return -1;  // more distinct seeds than the capacity, or a first call that would fix it at 0
+    v->ensure_initial_reset();
+    KParams &base = v->base;
+    const int G = (int)v->games.size();
+    if (!base.bank.slots) {
+        v->bank_capacity = std::max(count, capacity);
+        v->d_bank_seeds = dev_alloc<int32_t>((size_t)v->bank_capacity);
+        v->d_bank_count = dev_alloc<int32_t>(1);
+        // a banked step lists its resets as a step with final outputs does (launch_banked_step)
+        base.bank_level_end = dev_alloc<uint8_t>((size_t)v->num_envs);
+        if (!v->d_reset_list) {
+            v->d_reset_list = dev_alloc<int32_t>((size_t)v->num_envs);
+            base.reset_list = v->d_reset_list;
+        }
+        // per game: int32 usable (16 B) | EnvHdr | Entity[ENT_CAP] | grid[GRID_CAP] | MT19937 | persistent scratch
+        size_t total = 0;
+        for (const GameVTable *g : v->games) {
+            LevelBank b{};
+            b.ents_off = BANK_SLOT_HEAD + (int)sizeof(EnvHdr);
+            b.grid_off = b.ents_off + g->ent_cap * (int)sizeof(Entity);
+            b.rng_off = b.grid_off + ((g->grid_cap * (int)sizeof(int16_t) + 15) & ~15);
+            b.scratch_off = b.rng_off + (int)sizeof(MT19937);
+            b.slot_bytes = b.scratch_off + ((g->persist_scratch_words * (int)sizeof(int32_t) + 15) & ~15);
+            b.options = base.options;
+            b.seeds = v->d_bank_seeds;
+            b.count = v->d_bank_count;
+            b.slots = reinterpret_cast<unsigned char *>(total);  // offset until the allocation below
+            total += (size_t)v->bank_capacity * b.slot_bytes;
+            v->banks.push_back(b);
+        }
+        unsigned char *slots = dev_alloc<unsigned char>(total);
+        for (LevelBank &b : v->banks) b.slots = slots + reinterpret_cast<size_t>(b.slots);
+        v->bank_bytes = (int64_t)total + (int64_t)v->bank_capacity * (int64_t)sizeof(int32_t) + (int64_t)sizeof(int32_t);
+        // set last: a non-null slots pointer is what selects the bank's kernels
+        base.bank = v->banks[0];
+        base.bank.slots = slots;
+#ifndef PG_HOSTSIM
+        CUDA_CHECK(cudaDeviceSynchronize());  // dev_alloc's memsets ran on the legacy stream
+#endif
+    }
+    // staging of the build's warps (a level generated at the env's own capacities), bounded by a fixed budget
+    const size_t stage_bytes = bank_stage_bytes(base);
+    int warps = (int)std::min<size_t>((size_t)std::max(n, 1), std::max<size_t>(((size_t)256 << 20) / stage_bytes, 1));
+#ifndef PG_HOSTSIM
+    warps = std::min(warps, v->max_logic_blocks * kLogicEnvsPerBlock);
+    unsigned char *stage = nullptr;
+    CUDA_CHECK(cudaMalloc((void **)&stage, (size_t)warps * stage_bytes));
+    // ordered behind every step issued so far, and every later step behind the rebuild
+    CUDA_CHECK(cudaMemcpyAsync(v->d_bank_seeds, sorted.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, v->stream));
+#else
+    unsigned char *stage = (unsigned char *)calloc(stage_bytes, 1);
+    memcpy(v->d_bank_seeds, sorted.data(), (size_t)n * sizeof(int32_t));
+#endif
+    for (int g = 0; g < G; g++) {
+        KParams p = base;
+        p.assets = v->d_assets[g];
+        p.game_id = v->games[g]->id;
+        p.fixed_asset_seed = fnv1a(v->games[g]->name);
+        p.bank = v->banks[g];
+        LaunchCtx lc = v->lctx();
+        v->games[g]->bank_build(p, lc, stage, warps, n);
+    }
+#ifndef PG_HOSTSIM
+    const int32_t n_dev = n;
+    CUDA_CHECK(cudaMemcpyAsync(v->d_bank_count, &n_dev, sizeof(int32_t), cudaMemcpyHostToDevice, v->stream));
+    v->sync();  // the host sources above, then the staging
+    CUDA_CHECK(cudaFree(stage));
+#else
+    *v->d_bank_count = n;
+    free(stage);
+#endif
+    v->bank_levels = n;
+    return 0;
+}
+
+int pgb200_level_bank_info(libenv_env *handle, int *levels, int64_t *bytes) {
+    VecEnv *v = (VecEnv *)handle;
+    if (levels)
+        *levels = v->bank_levels;
+    if (bytes)
+        *bytes = v->bank_bytes;
     return 0;
 }
 

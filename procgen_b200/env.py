@@ -138,6 +138,7 @@ class BaseProcgenEnv:
         self._next_level_seeds = None
         self._final_outputs = None
         self._pause_mask = None
+        self._num_levels, self._start_level = num_levels, start_level
         self._consumer_slot = None
         self._graph_stepped = False   # act() has run inside a CUDA graph capture
         self._retired_consumers = []  # consumer buffers a captured graph may still write
@@ -420,6 +421,37 @@ class BaseProcgenEnv:
                 dev = torch.device("cuda", self.device_index)
                 self._pause_mask = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "|u1"), device=dev)
         return self._pause_mask
+
+    def build_level_bank(self, seeds=None, capacity: int = 0) -> None:
+        """Bank the levels of `seeds` (default: range(start_level, start_level + num_levels)) for every game of the
+        handle: a reset inside a step onto a banked seed copies the level generated here instead of generating it
+        again. Only speed changes: every output and state is the one a handle without a bank gives. The first call
+        fixes the capacity at max(len(seeds), capacity) distinct seeds, which must not be 0; a later call rebuilds
+        the bank in place (CUDA graphs captured after the first call see the rebuild), and an empty `seeds` empties
+        it. The rebuild is ordered behind every step issued before it, graph replays on the current stream
+        included. Raises ValueError for a seed outside [0, 2^31), more distinct seeds than the capacity, or a first
+        call with no seeds and no capacity."""
+        if seeds is None:
+            if self._num_levels == 0:
+                raise ValueError("build_level_bank(): num_levels == 0 plays unboundedly many levels; pass the seeds to bank")
+            seeds = range(self._start_level, self._start_level + self._num_levels)
+        self._refuse_in_capture("build_level_bank")
+        self._wait_for_replays()
+        arr = np.asarray(list(seeds), dtype=np.int64).reshape(-1)
+        if arr.size and (arr.min() < 0 or arr.max() >= 2 ** 31):
+            raise ValueError("build_level_bank(): every seed must be in [0, 2^31)")
+        arr = np.ascontiguousarray(arr.astype(np.int32))
+        ptr = arr.ctypes.data_as(C.POINTER(C.c_int32))
+        if self._lib.pgb200_build_level_bank(self._h, ptr, int(arr.size), int(capacity)) != 0:
+            raise ValueError(f"build_level_bank(): {len(np.unique(arr))} distinct seeds exceed the bank's capacity, or a "
+                             "first call has no seeds and capacity 0")
+
+    def level_bank_info(self) -> dict:
+        """{"levels": distinct seeds banked, "bytes": device memory the bank holds}; zeros without a bank."""
+        self._refuse_in_capture("level_bank_info")
+        levels, nbytes = C.c_int(0), C.c_int64(0)
+        self._lib.pgb200_level_bank_info(self._h, C.byref(levels), C.byref(nbytes))
+        return {"levels": levels.value, "bytes": nbytes.value}
 
     def callmethod(self, method: str, *args, **kwargs):
         return getattr(self, method)(*args, **kwargs)

@@ -57,7 +57,8 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_kernel_timing_begin", "pgb200_kernel_timing_end", "get_state", "set_state", "pgb200_set_launch_shape",
            "pgb200_frame_info", "pgb200_set_rgb_mirror", "pgb200_mirror_parity",
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
-           "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask"]
+           "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
+           "pgb200_build_level_bank", "pgb200_level_bank_info"]
 
 _lib = None
 
@@ -81,6 +82,10 @@ def bind(lib):
     lib.pgb200_get_final_outputs.restype = C.c_int
     lib.pgb200_get_pause_mask.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8))]
     lib.pgb200_get_pause_mask.restype = C.c_int
+    lib.pgb200_build_level_bank.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int]
+    lib.pgb200_build_level_bank.restype = C.c_int
+    lib.pgb200_level_bank_info.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int64)]
+    lib.pgb200_level_bank_info.restype = C.c_int
     lib.pgb200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     lib.pgb200_set_stream.restype = None
     lib.pgb200_get_errors.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]

@@ -1,6 +1,7 @@
 """Per-env logic-kernel duration at steady state, split into steps that ended an episode (level
 generation) and ordinary steps. Needs PGB200_DEBUG_TIMING=1 (set here). One JSON line per game.
-usage: python tools/gpu_reset_cost.py [envs] [desync_steps] [game:mode ...]"""
+usage: python tools/gpu_reset_cost.py [--num-levels L] [--bank] [envs] [desync_steps] [game:mode ...]
+--num-levels L plays the levels [0, L) (default 0: unboundedly many); --bank also banks them (build_level_bank)."""
 import json
 import os
 import sys
@@ -12,12 +13,21 @@ import torch
 
 from procgen_b200 import ENV_NAMES, ProcgenGym3Env
 
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 32768
-desync = int(sys.argv[2]) if len(sys.argv) > 2 else 600
-games = sys.argv[3:] or [g + ":hard" for g in ENV_NAMES]
+args = sys.argv[1:]
+num_levels, bank = 0, "--bank" in args
+if "--num-levels" in args:
+    i = args.index("--num-levels")
+    num_levels = int(args[i + 1])
+    del args[i:i + 2]
+args = [a for a in args if a != "--bank"]
+n = int(args[0]) if len(args) > 0 else 32768
+desync = int(args[1]) if len(args) > 1 else 600
+games = args[2:] or [g + ":hard" for g in ENV_NAMES]
 for gm in games:
     game, mode = gm.split(":")
-    env = ProcgenGym3Env(n, game, distribution_mode=mode, num_levels=0, rand_seed=0)
+    env = ProcgenGym3Env(n, game, distribution_mode=mode, num_levels=num_levels, rand_seed=0)
+    if bank:
+        env.build_level_bank()
     g = torch.Generator(device="cuda").manual_seed(0)
     acts = torch.randint(0, 15, (64, n), device="cuda", dtype=torch.int32, generator=g)
     for t in range(desync):
@@ -38,7 +48,7 @@ for gm in games:
     kt = env.kernel_timing_end()
     r = np.concatenate(r_c)
     q = np.concatenate(n_c)
-    out = {"game": game, "mode": mode, "envs": n, "resets_per_step": len(r) / 16.0,
+    out = {"game": game, "mode": mode, "envs": n, "num_levels": num_levels, "bank": bank, "resets_per_step": len(r) / 16.0,
            "reset_cycles": {"mean": float(r.mean()) if len(r) else None, "p50": float(np.percentile(r, 50)) if len(r) else None,
                             "p99": float(np.percentile(r, 99)) if len(r) else None, "max": float(r.max()) if len(r) else None},
            "step_cycles": {"mean": float(q.mean()), "p50": float(np.percentile(q, 50)), "p99": float(np.percentile(q, 99)), "max": float(q.max())},
