@@ -400,18 +400,22 @@ __global__ void camera_kernel(KParams p) {
 }
 #endif
 
-// the setup + render kernels' phases as plain loops (host debug harness; also documents the phase order)
-template <class G, int VIEW, class Frame>
-void render_env_serial(const KParams &p, int env, Frame &f) {
+// the setup + render kernels' phases as plain loops (host debug harness; also documents the phase order). PASS: see
+// render_kernel; in pass 1 the frame of an env whose level ended goes to final_rgb.
+template <class G, int VIEW, int PASS>
+void render_env_serial(const KParams &p, int env) {
+    using Frame = typename FrameFor<G, VIEW>::type;
     using Setup = typename FrameFor<G, VIEW>::setup;
     using Shared = typename FrameFor<G, VIEW>::shared;
+    static thread_local Frame *f = new Frame;
     Setup &s = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
     env_setup_frame<G, Setup>(p, env, s, 0, 1);
-    static_cast<Shared &>(f) = static_cast<const Shared &>(s);
-    env_stage_tiles_serial<Frame>(p, f);
-    for (int w = 0; w < 4; w++) env_render_compose<G, Frame>(p, f, w, 4, 0, 1);  // the device's row ownership, one lane per owner
-    uint32_t *out = reinterpret_cast<uint32_t *>(p.rgb + (size_t)env * (RES_W * RES_H * 3));
-    for (int g = 0; g < RES_W * RES_H / 4; g++) Raster<G, Frame>::pack_quad(f.fb + 4 * g, out + 3 * g);
+    static_cast<Shared &>(*f) = static_cast<const Shared &>(s);
+    env_stage_tiles_serial<Frame>(p, *f);
+    for (int w = 0; w < 4; w++) env_render_compose<G, Frame>(p, *f, w, 4, 0, 1);  // the device's row ownership, one lane per owner
+    uint8_t *rgb = PASS == 1 && p.level_end[env] != 0 ? p.final_rgb : p.rgb;
+    uint32_t *out = reinterpret_cast<uint32_t *>(rgb + (size_t)env * (RES_W * RES_H * 3));
+    for (int g = 0; g < RES_W * RES_H / 4; g++) Raster<G, Frame>::pack_quad(f->fb + 4 * g, out + 3 * g);
 }
 
 struct LaunchCtx {
@@ -419,12 +423,14 @@ struct LaunchCtx {
     cudaStream_t stream;
     cudaStream_t logic_stream;  // null, or a higher-priority stream the logic kernel goes to (then `link` orders render behind it)
     cudaEvent_t link;
-    unsigned int *ticket;     // work counter of this launch slot (one per in-flight logic kernel)
     int max_logic_blocks;     // SM count x resident CTAs per SM
     int num_sms;              // SM count: sizes the machine-filling grids of a final-outputs step's phase B
     int render_smem_floor;    // dynamic shared memory requested per render CTA is at least this (co-residency knob)
     cudaEvent_t *tev;         // optional: 4 events (before logic, after it, after setup, after render) for kernel timing
 #endif
+    // work counter of this launch slot (one per in-flight logic kernel); a two-phase step keeps its list's count and
+    // phase B's ticket in the next two words
+    unsigned int *ticket;
     int64_t *launch_counter;
 };
 
@@ -446,222 +452,177 @@ int prepare_render_smem(const LaunchCtx &lc) {
     }
     return bytes;
 }
-#endif
 
-#ifndef PG_HOSTSIM
-// One (game, env chunk) launch of a step with final outputs: two phases on the chunk's stream.
-//   A  logic (FINAL: listing the envs whose level ends), setup, render (their frames to final_rgb)
-//   B  finish (their resets), setup and render over the list: their next level's first frame to rgb
-// ticket[0] is phase A's ticket, ticket[1] the list's count and ticket[2] phase B's ticket: one memset clears
-// all three. Phase B's grids are fixed (machine-filling) and read the count on the device, so nothing waits for
-// the host and the step stays capturable. Everything goes to lc.stream (a priority-split logic stream would
-// let the next launch that shares this ticket slot clear it under phase B). PAUSE: phase A skips paused envs, and
-// phase B, which only sees the list, needs no variant.
-template <class G, int VIEW, bool PAUSE, bool BANK>
-void launch_final_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
-    KParams q = p;
-    q.reset_count = lc.ticket + 1;
-    const int render_a = prepare_render_smem<G, VIEW, 1, PAUSE>(lc);
-    const int render_b = prepare_render_smem<G, VIEW, 2>(lc);
-    const int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
-    const int setup_b = setup_blocks < lc.num_sms * PG_SETUP_MIN_BLOCKS ? setup_blocks : lc.num_sms * PG_SETUP_MIN_BLOCKS;
-    const int render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
-    const int render_blocks_b = p.env_count < render_fit ? p.env_count : render_fit;
-    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, 3 * sizeof(unsigned int), lc.stream));
-    logic_kernel<G, false, false, true, PAUSE><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
-    setup_kernel<G, VIEW, false, PAUSE><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(q);
-    render_kernel<G, VIEW, 1, PAUSE><<<p.env_count, kRenderThreads, render_a, lc.stream>>>(q);
-    finish_kernel<G, BANK><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
-    setup_kernel<G, VIEW, true><<<setup_b, kSetupThreads, 0, lc.stream>>>(q);
-    render_kernel<G, VIEW, 2><<<render_blocks_b, kRenderThreads, render_b, lc.stream>>>(q);
-    CUDA_CHECK(cudaGetLastError());
-    (*lc.launch_counter) += 6;
+// grid of the persistent logic and finish kernels: one warp per env, at most what the machine holds at once
+static inline int logic_grid(const KParams &p, const LaunchCtx &lc) {
+    const int blocks = (p.env_count + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
+    return blocks < lc.max_logic_blocks ? blocks : lc.max_logic_blocks;
 }
 #endif
 
-#ifndef PG_HOSTSIM
-// One (game, env chunk) launch of a plain step on a handle with a level bank and without final outputs. Its resets
-// run in a kernel of their own, so that the step itself runs the logic kernel it always runs (its stack frame and
-// registers stay those of the step, which must fit the push_obj / sub_step recursion): phase A of a step with final
-// outputs (level_end to the handle's own bank_level_end), the finish kernel over its list, where the resets copy
-// their levels from the bank, then one setup and one render over the launch's envs. Tickets as launch_final_step.
-template <class G, int VIEW, bool PAUSE>
-void launch_banked_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
-    KParams q = p;
-    q.level_end = p.bank_level_end;
-    q.reset_count = lc.ticket + 1;
-    const int render_smem = prepare_render_smem<G, VIEW, 0, PAUSE>(lc);
-    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, 3 * sizeof(unsigned int), lc.stream));
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[0], lc.stream));
-    logic_kernel<G, false, false, true, PAUSE><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket);
-    finish_kernel<G, true><<<logic_blocks, kLogicThreads, 0, lc.stream>>>(q, lc.ticket + 2);
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
-    setup_kernel<G, VIEW, false, PAUSE><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
-    render_kernel<G, VIEW, 0, PAUSE><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
-    if (lc.tev)
-        CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
-    CUDA_CHECK(cudaGetLastError());
-    (*lc.launch_counter) += 4;
-}
-#endif
+// The phases of a step. Each launches its kernels on the launch's stream or, in the host debug build, runs the same
+// per-env code as a loop over the launch's envs or over the reset list.
 
+// logic: clears the launch's ticket, then runs the logic kernel over the launch's envs. FINAL: phase A of a two-phase
+// step, which lists the envs whose level ends in p.reset_list and clears the list's count and phase B's ticket with
+// its own. A two-phase step stays on lc.stream: a priority-split logic stream would let the next launch that shares
+// this ticket slot clear it under phase B. A one-phase step's logic kernel may go to that stream (PGB200_PRIORITY_SPLIT).
+template <class G, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE>
+void logic_phase(const KParams &p, const LaunchCtx &lc) {
+    constexpr size_t kTicketBytes = (FINAL ? 3 : 1) * sizeof(unsigned int);
 #ifndef PG_HOSTSIM
-// One (game, env chunk) launch of a plain step (or of the initial reset): logic, setup, render. PAUSE: the
-// instantiations that skip the envs the handle's pause mask holds still.
-template <class G, bool INIT, int VIEW, bool PAUSE>
-void launch_plain_step(const KParams &p, const LaunchCtx &lc, int logic_blocks) {
-    // Shared memory per render CTA: the frame, or more when the handle asks for fewer resident
-    // render CTAs per SM. At 8 CTAs x 128 threads x 64 registers the render kernel owns the whole
-    // register file of an SM and no logic-kernel block of another env chunk can run beside it;
-    // capping its residency trades a little render speed for real overlap of the two kernels.
-    const int render_smem = prepare_render_smem<G, VIEW, 0, PAUSE>(lc);
-    cudaStream_t ls = lc.logic_stream ? lc.logic_stream : lc.stream;
-    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, sizeof(unsigned int), ls));
+    const cudaStream_t ls = !FINAL && lc.logic_stream ? lc.logic_stream : lc.stream;
+    CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, kTicketBytes, ls));
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[0], ls));
-    if (!INIT && p.next_level_seed)
-        logic_kernel<G, false, true, false, PAUSE><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
-    else
-        logic_kernel<G, INIT, false, false, PAUSE><<<logic_blocks, kLogicThreads, 0, ls>>>(p, lc.ticket);
-    if (lc.logic_stream) {
+    logic_kernel<G, INIT, LEVEL_CHOICE, FINAL, PAUSE><<<logic_grid(p, lc), kLogicThreads, 0, ls>>>(p, lc.ticket);
+    CUDA_CHECK(cudaGetLastError());
+    if (ls != lc.stream) {
         CUDA_CHECK(cudaEventRecord(lc.link, ls));
         CUDA_CHECK(cudaStreamWaitEvent(lc.stream, lc.link, 0));
     }
+#else
+    using Frame = typename FrameFor<G>::type;
+    memset(lc.ticket, 0, kTicketBytes);
+    for (int i = 0; i < p.env_count; i++) {
+        const int env = p.env_first + i * p.env_step;
+        if (INIT)
+            env_init_logic<G, Frame>(p, env);
+        else if (PAUSE && env_pause_logic<FINAL>(p, env)) {
+        } else if (FINAL) {
+            if (env_step_logic_final<G, Frame>(p, env))
+                p.reset_list[(*p.reset_count)++] = env;
+        } else
+            env_step_logic<G, Frame, LEVEL_CHOICE>(p, env);
+    }
+#endif
+}
+
+// finish: phase B's resets, the finish kernel over the envs phase A listed. BANK: they copy their levels from the
+// bank where it holds them.
+template <class G, bool BANK>
+void finish_phase(const KParams &p, const LaunchCtx &lc) {
+#ifndef PG_HOSTSIM
+    finish_kernel<G, BANK><<<logic_grid(p, lc), kLogicThreads, 0, lc.stream>>>(p, lc.ticket + 2);
+    CUDA_CHECK(cudaGetLastError());
+#else
+    (void)lc;
+    using Frame = typename FrameFor<G>::type;
+    for (unsigned int j = 0; j < *p.reset_count; j++) env_finish_logic<G, Frame, BANK>(p, p.reset_list[j]);
+#endif
+}
+
+// frames: the setup kernel, then the render kernel of pass PASS, between kernel-timing events 1 to 3 (the runtime
+// gives a step with final outputs none). PASS 0 and 1 cover the launch's envs, and PAUSE leaves the paused ones'
+// frames as they are. PASS 2 covers the envs phase A listed: its grids are fixed (machine-filling) and read the
+// list's count on the device, so nothing waits for the host and the step stays capturable.
+template <class G, int VIEW, int PASS, bool PAUSE>
+void frames_phase(const KParams &p, const LaunchCtx &lc) {
+    constexpr bool LIST = PASS == 2;
+#ifndef PG_HOSTSIM
+    const int render_smem = prepare_render_smem<G, VIEW, PASS, PAUSE>(lc);
+    int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
+    int render_blocks = p.env_count;
+    if (LIST) {
+        const int setup_fit = lc.num_sms * PG_SETUP_MIN_BLOCKS, render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
+        setup_blocks = setup_blocks < setup_fit ? setup_blocks : setup_fit;
+        render_blocks = render_blocks < render_fit ? render_blocks : render_fit;
+    }
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
-    setup_kernel<G, VIEW, false, PAUSE><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
+    setup_kernel<G, VIEW, LIST, PAUSE><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(p);
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
-    render_kernel<G, VIEW, 0, PAUSE><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
+    render_kernel<G, VIEW, PASS, PAUSE><<<render_blocks, kRenderThreads, render_smem, lc.stream>>>(p);
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
     CUDA_CHECK(cudaGetLastError());
-    (*lc.launch_counter) += 3;
-}
+#else
+    (void)lc;
+    if (LIST) {
+        for (unsigned int j = 0; j < *p.reset_count; j++) render_env_serial<G, VIEW, PASS>(p, p.reset_list[j]);
+        return;
+    }
+    for (int i = 0; i < p.env_count; i++) {
+        const int env = p.env_first + i * p.env_step;
+        if (!(PAUSE && p.paused[env]))
+            render_env_serial<G, VIEW, PASS>(p, env);
+    }
 #endif
+}
+
+// One (game, env chunk) launch of a step (or of the initial reset), as its phases:
+//   initial reset, plain step                logic, frames(0)
+//   level bank, without final outputs        logic (phase A), finish, frames(0)
+//   final outputs, with or without a bank    logic (phase A), frames(1), finish, frames(2)
+// A final-outputs step's phase A renders the final frames of the envs whose level ends, to final_rgb; phase B renders
+// the first frames of their next levels. A banked step without final outputs also runs its resets in the finish
+// kernel, so that its logic kernel is one that steps always run (its stack frame and registers stay those of the
+// step, which must fit the push_obj / sub_step recursion); phase A's level_end goes to the handle's bank_level_end.
+// PAUSE: the instantiations that skip the envs the handle's pause mask holds still; phase B, which only sees the
+// list, needs none.
+template <class G, int VIEW, bool INIT, bool PAUSE, bool FINAL, bool BANK>
+void launch_step(const KParams &p, const LaunchCtx &lc) {
+    KParams q = p;  // what the phases of a two-phase step see
+    q.reset_count = lc.ticket + 1;
+    if constexpr (BANK && !FINAL)
+        q.level_end = p.bank_level_end;
+    if constexpr (FINAL || BANK)
+        logic_phase<G, false, false, true, PAUSE>(q, lc);
+    else if (!INIT && p.next_level_seed)
+        logic_phase<G, false, true, false, PAUSE>(p, lc);
+    else
+        logic_phase<G, INIT, false, false, PAUSE>(p, lc);
+    if constexpr (FINAL) {
+        frames_phase<G, VIEW, 1, PAUSE>(q, lc);
+        finish_phase<G, BANK>(q, lc);
+        frames_phase<G, VIEW, 2, false>(q, lc);
+    } else {
+        if constexpr (BANK)
+            finish_phase<G, true>(q, lc);
+        frames_phase<G, VIEW, 0, PAUSE>(p, lc);
+    }
+    (*lc.launch_counter) += FINAL ? 6 : BANK ? 4 : 3;
+}
 
 template <class G, bool INIT, int VIEW>
 void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
-    using Frame = typename FrameFor<G, VIEW>::type;
     if (p.env_count <= 0)
         return;
-#ifndef PG_HOSTSIM
-    int logic_blocks = (p.env_count + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
-    if (logic_blocks > lc.max_logic_blocks)
-        logic_blocks = lc.max_logic_blocks;
     if constexpr (INIT) {
-        launch_plain_step<G, true, VIEW, false>(p, lc, logic_blocks);
-    } else if (p.bank.slots) {
-        if (p.level_end && p.pause)
-            launch_final_step<G, VIEW, true, true>(p, lc, logic_blocks);
-        else if (p.level_end)
-            launch_final_step<G, VIEW, false, true>(p, lc, logic_blocks);
-        else if (p.pause)
-            launch_banked_step<G, VIEW, true>(p, lc, logic_blocks);
-        else
-            launch_banked_step<G, VIEW, false>(p, lc, logic_blocks);
-    } else {
-        // a handle without a pause mask or a level bank runs exactly the kernels it ran before they existed
-        if (p.level_end && p.pause)
-            launch_final_step<G, VIEW, true, false>(p, lc, logic_blocks);
-        else if (p.level_end)
-            launch_final_step<G, VIEW, false, false>(p, lc, logic_blocks);
-        else if (p.pause)
-            launch_plain_step<G, false, VIEW, true>(p, lc, logic_blocks);
-        else
-            launch_plain_step<G, false, VIEW, false>(p, lc, logic_blocks);
-    }
-#else
-    static thread_local Frame *f = new Frame;
-    if (!INIT && !p.level_end && p.bank.slots) {
-        // the serial twin of launch_banked_step
-        unsigned int count = 0;
-        KParams q = p;
-        q.level_end = p.bank_level_end;
-        q.reset_count = &count;
-        for (int b = 0; b < p.env_count; b++) {
-            const int env = p.env_first + b * p.env_step;
-            if (p.pause && env_pause_logic<true>(q, env))
-                continue;
-            if (env_step_logic_final<G, Frame>(q, env))
-                q.reset_list[count++] = env;
-        }
-        for (unsigned int j = 0; j < count; j++) env_finish_logic<G, Frame, true>(q, q.reset_list[j]);
-        for (int b = 0; b < p.env_count; b++) {
-            const int env = p.env_first + b * p.env_step;
-            if (!(p.pause && p.paused[env]))
-                render_env_serial<G, VIEW, Frame>(p, env, *f);
-        }
-        (*lc.launch_counter) += 4;
+        launch_step<G, VIEW, true, false, false, false>(p, lc);
         return;
     }
-    if (!INIT && p.level_end) {
-        // the serial twin of launch_final_step's two phases
-        unsigned int count = 0;
-        KParams q = p;
-        q.reset_count = &count;
-        KParams fin = q;
-        fin.rgb = p.final_rgb;
-        for (int b = 0; b < p.env_count; b++) {
-            const int env = p.env_first + b * p.env_step;
-            if (p.pause && env_pause_logic<true>(q, env))
-                continue;  // setup and render skip it (q.paused[env]), and it never enters the list
-            const bool ended = env_step_logic_final<G, Frame>(q, env);
-            if (ended)
-                q.reset_list[count++] = env;
-            render_env_serial<G, VIEW, Frame>(ended ? fin : q, env, *f);
-        }
-        for (unsigned int j = 0; j < count; j++) {
-            if (p.bank.slots)
-                env_finish_logic<G, Frame, true>(q, q.reset_list[j]);
-            else
-                env_finish_logic<G, Frame>(q, q.reset_list[j]);
-            render_env_serial<G, VIEW, Frame>(q, q.reset_list[j], *f);
-        }
-        (*lc.launch_counter) += 6;
-        return;
+    // a handle without a pause mask, final outputs or a level bank runs exactly the kernels it ran before they existed
+    switch ((p.pause ? 1 : 0) | (p.level_end ? 2 : 0) | (p.bank.slots ? 4 : 0)) {
+    case 0: launch_step<G, VIEW, false, false, false, false>(p, lc); break;
+    case 1: launch_step<G, VIEW, false, true, false, false>(p, lc); break;
+    case 2: launch_step<G, VIEW, false, false, true, false>(p, lc); break;
+    case 3: launch_step<G, VIEW, false, true, true, false>(p, lc); break;
+    case 4: launch_step<G, VIEW, false, false, false, true>(p, lc); break;
+    case 5: launch_step<G, VIEW, false, true, false, true>(p, lc); break;
+    case 6: launch_step<G, VIEW, false, false, true, true>(p, lc); break;
+    case 7: launch_step<G, VIEW, false, true, true, true>(p, lc); break;
     }
-    for (int b = 0; b < p.env_count; b++) {
-        int env = p.env_first + b * p.env_step;
-        if (INIT)
-            env_init_logic<G, Frame>(p, env);
-        else if (p.pause && env_pause_logic<false>(p, env))
-            continue;  // setup and render skip it (p.paused[env])
-        else if (p.next_level_seed)
-            env_step_logic<G, Frame, true>(p, env);
-        else
-            env_step_logic<G, Frame>(p, env);
-        render_env_serial<G, VIEW, Frame>(p, env, *f);
-    }
-    (*lc.launch_counter) += 3;
-#endif
 }
 
 template <class G, int VIEW>
 void launch_observe_only(const KParams &p, const LaunchCtx &lc) {
-    using Frame = typename FrameFor<G, VIEW>::type;
     if (p.env_count <= 0)
         return;
 #ifndef PG_HOSTSIM
-    const int render_smem = prepare_render_smem<G, VIEW>(lc);
     camera_kernel<G><<<p.env_count, 32, 0, lc.stream>>>(p);
-    setup_kernel<G, VIEW><<<(p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32), kSetupThreads, 0, lc.stream>>>(p);
-    render_kernel<G, VIEW><<<p.env_count, kRenderThreads, render_smem, lc.stream>>>(p);
     CUDA_CHECK(cudaGetLastError());
 #else
-    static thread_local Frame *f = new Frame;
+    using Frame = typename FrameFor<G>::type;
     for (int b = 0; b < p.env_count; b++) {
         int env = p.env_first + b * p.env_step;
         Ctx c = make_ctx(p, env);
         Raster<G, Frame>::prepare_camera(c);
         write_step_outputs(p, env, *c.h);
-        render_env_serial<G, VIEW, Frame>(p, env, *f);
     }
 #endif
+    frames_phase<G, VIEW, 0, false>(p, lc);
     (*lc.launch_counter) += 2;
 }
 

@@ -174,6 +174,13 @@ void copy_to_dev(void *dst, const void *src, size_t bytes) {
     memcpy(dst, src, bytes);
 #endif
 }
+void copy_from_dev(void *dst, const void *src, size_t bytes) {
+#ifndef PG_HOSTSIM
+    CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+#else
+    memcpy(dst, src, bytes);
+#endif
+}
 
 // vecgame.cpp:156-167: system-independent hash of the game name
 static int32_t fnv1a(const char *str) {
@@ -241,12 +248,12 @@ struct VecEnv {
     SpriteDesc *d_tile_sprites = nullptr;
     uint32_t *d_lvl_seeds = nullptr;
     int32_t *d_action = nullptr;
-    int32_t *d_next_level_seed = nullptr;   // allocated by the first pgb200_get_next_level_seeds
-    // allocated by the first pgb200_get_final_outputs: base.final_rgb, base.level_end and the pending-reset list
-    int32_t *d_reset_list = nullptr;
-    // allocated by the first pgb200_get_pause_mask: the caller's mask (base.pause) and what the logic kernel
-    // recorded of it for the step's later kernels (base.paused)
-    uint8_t *d_pause = nullptr, *d_paused = nullptr;
+    // The opt-in per-env arrays live in `base`, allocated by the first request for them (opt_in_array):
+    // next_level_seed by pgb200_get_next_level_seeds; final_rgb and level_end by pgb200_get_final_outputs;
+    // pause (the caller's mask, d_pause) and paused (what the logic kernel recorded of it for the step's later
+    // kernels) by pgb200_get_pause_mask; bank_level_end by the first pgb200_build_level_bank. reset_list, the
+    // pending-reset list of a two-phase step, by whichever of final outputs and the bank comes first.
+    uint8_t *d_pause = nullptr;
     // allocated by the first pgb200_build_level_bank: bank_capacity slots per game of the list, sized by the game
     // (banks[g], one allocation at base.bank.slots), the sorted seed list they share and its length on the device
     std::vector<LevelBank> banks;
@@ -318,12 +325,12 @@ struct VecEnv {
         lc.stream = stream;
         lc.logic_stream = nullptr;
         lc.link = nullptr;
-        lc.ticket = d_tickets;
         lc.max_logic_blocks = max_logic_blocks;
         lc.num_sms = num_sms;
         lc.render_smem_floor = render_smem_floor;
         lc.tev = nullptr;
 #endif
+        lc.ticket = d_tickets;
         lc.launch_counter = &launches;
         return lc;
     }
@@ -381,6 +388,7 @@ struct VecEnv {
                 if (base.bank.slots)
                     p.bank = banks[g];
                 LaunchCtx lc = lctx();
+                lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
 #ifndef PG_HOSTSIM
                 if (nstreams) {
                     lc.stream = aux[k % nstreams];
@@ -389,7 +397,6 @@ struct VecEnv {
                         lc.link = ev_link[k % nstreams];
                     }
                 }
-                lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
                 if (timing && !base.level_end && tev_used + 4 <= tev_pool.size()) {
                     lc.tev = &tev_pool[tev_used];
                     tev_used += 4;
@@ -463,6 +470,33 @@ struct VecEnv {
     void refuse_in_capture(const char *what) {
         if (capturing())
             pg_fatal("%s cannot run while the handle's stream is capturing a CUDA graph\n", what);
+    }
+
+    // The start of an entry point that hands out an opt-in array: false (the entry point returns -1) while the
+    // handle's stream captures, unless the array is already allocated (`allocated`) and the initial reset has run,
+    // since either would invalidate the caller's capture. Then the initial reset.
+    bool begin_opt_in(bool allocated) {
+        if ((!initial_reset_done || !allocated) && capturing())
+            return false;
+        ensure_initial_reset();
+        return true;
+    }
+
+    // An opt-in per-env array of `per_env` elements per env, allocated at the first request (ptr null) with every
+    // byte set to `fill` on the handle's stream, which completes before the caller uses it from any stream
+    template <class T>
+    void opt_in_array(T *&ptr, size_t per_env, int fill) {
+        if (ptr)
+            return;
+        const size_t bytes = (num_envs ? (size_t)num_envs : 1) * per_env * sizeof(T);
+#ifndef PG_HOSTSIM
+        CUDA_CHECK(cudaMalloc((void **)&ptr, bytes));
+        CUDA_CHECK(cudaMemsetAsync(ptr, fill, bytes, stream));
+#else
+        ptr = (T *)malloc(bytes);
+        memset(ptr, fill, bytes);
+#endif
+        sync();
     }
 
     void set_device() {
@@ -671,7 +705,6 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
             v->render_smem_floor = (227 * 1024) / render_ctas - 1024 - 16;
             v->render_smem_floor &= ~15;
         }
-        CUDA_CHECK(cudaMalloc((void **)&v->d_tickets, VecEnv::kMaxTickets * VecEnv::kTicketWords * sizeof(unsigned int)));
         v->d_consumer_slot = dev_alloc<int32_t>(1);
         v->base.consumer_slot_dev = v->d_consumer_slot;
     }
@@ -685,6 +718,7 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
 #else
     v->device = -1;
 #endif
+    v->d_tickets = dev_alloc<unsigned int>(VecEnv::kMaxTickets * VecEnv::kTicketWords);
 
     // ---- assets
     std::string pack_path = resource_root;
@@ -868,29 +902,30 @@ static void host_free(void *ptr) {
 #endif
 }
 
+// device -> host on the handle's stream, ordered behind its kernels (host build: memcpy)
+static void copy_from_dev_async(VecEnv *v, void *dst, const void *src, size_t bytes) {
+#ifndef PG_HOSTSIM
+    CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, v->stream));
+#else
+    (void)v;
+    memcpy(dst, src, bytes);
+#endif
+}
+
 static void fetch_to_host(VecEnv *v) {
     const size_t N = (size_t)v->num_envs;
     const KParams &p = v->base;
     const size_t frame = RES_W * RES_H * 3;
     uint8_t *rgb_dst = v->ob_direct ? (uint8_t *)v->h_ob[0] : v->st_rgb;
-#ifndef PG_HOSTSIM
     if (!v->rgb_copy_enqueued)
-        CUDA_CHECK(cudaMemcpyAsync(rgb_dst, p.rgb, N * frame, cudaMemcpyDeviceToHost, v->stream));
+        copy_from_dev_async(v, rgb_dst, p.rgb, N * frame);
     v->rgb_copy_enqueued = false;
-    CUDA_CHECK(cudaMemcpyAsync(v->st_rew, p.rew, N * sizeof(float), cudaMemcpyDeviceToHost, v->stream));
-    CUDA_CHECK(cudaMemcpyAsync(v->st_first, p.first, N, cudaMemcpyDeviceToHost, v->stream));
-    CUDA_CHECK(cudaMemcpyAsync(v->st_prev_seed, p.info_prev_level_seed, N * 4, cudaMemcpyDeviceToHost, v->stream));
-    CUDA_CHECK(cudaMemcpyAsync(v->st_prev_complete, p.info_prev_level_complete, N, cudaMemcpyDeviceToHost, v->stream));
-    CUDA_CHECK(cudaMemcpyAsync(v->st_seed, p.info_level_seed, N * 4, cudaMemcpyDeviceToHost, v->stream));
-    CUDA_CHECK(cudaStreamSynchronize(v->stream));
-#else
-    memcpy(rgb_dst, p.rgb, N * frame);
-    memcpy(v->st_rew, p.rew, N * sizeof(float));
-    memcpy(v->st_first, p.first, N);
-    memcpy(v->st_prev_seed, p.info_prev_level_seed, N * 4);
-    memcpy(v->st_prev_complete, p.info_prev_level_complete, N);
-    memcpy(v->st_seed, p.info_level_seed, N * 4);
-#endif
+    copy_from_dev_async(v, v->st_rew, p.rew, N * sizeof(float));
+    copy_from_dev_async(v, v->st_first, p.first, N);
+    copy_from_dev_async(v, v->st_prev_seed, p.info_prev_level_seed, N * 4);
+    copy_from_dev_async(v, v->st_prev_complete, p.info_prev_level_complete, N);
+    copy_from_dev_async(v, v->st_seed, p.info_level_seed, N * 4);
+    v->sync();
     if (!v->ob_direct)
         for (size_t e = 0; e < N; e++) memcpy(v->h_ob[e], v->st_rgb + e * frame, frame);
     memcpy(v->h_rew, v->st_rew, N * sizeof(float));
@@ -1000,12 +1035,12 @@ void libenv_close(libenv_env *handle) {
     dev_free(v->d_tile_index);
     dev_free(v->d_tile_sprites);
     dev_free(v->d_action);
-    dev_free(v->d_next_level_seed);
+    dev_free(p.next_level_seed);
     dev_free(p.final_rgb);
     dev_free(p.level_end);
-    dev_free(v->d_reset_list);
+    dev_free(p.reset_list);
     dev_free(v->d_pause);
-    dev_free(v->d_paused);
+    dev_free(p.paused);
     dev_free(p.bank.slots);
     dev_free(p.bank_level_end);
     dev_free(v->d_bank_seeds);
@@ -1024,11 +1059,7 @@ void libenv_close(libenv_env *handle) {
 #ifndef PG_HOSTSIM
     for (cudaEvent_t e : v->tev_pool) cudaEventDestroy(e);
 #endif
-#ifndef PG_HOSTSIM
-    if (v->d_tickets)
-        cudaFree(v->d_tickets);
-
-#endif
+    dev_free(v->d_tickets);
     for (auto a : v->d_assets) dev_free(a);
     host_free(v->st_rgb);
 #ifndef PG_HOSTSIM
@@ -1087,52 +1118,21 @@ int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *
 int pgb200_get_next_level_seeds(libenv_env *handle, int32_t **out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if ((!v->initial_reset_done || !v->d_next_level_seed) && v->capturing())
+    if (!v->begin_opt_in(v->base.next_level_seed != nullptr))
         return -1;
-    v->ensure_initial_reset();
-    if (!v->d_next_level_seed) {
-        const size_t N = (size_t)v->num_envs;
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaMalloc((void **)&v->d_next_level_seed, (N ? N : 1) * sizeof(int32_t)));
-        CUDA_CHECK(cudaMemsetAsync(v->d_next_level_seed, 0xff, N * sizeof(int32_t), v->stream));  // every entry -1
-        // complete before the caller writes, from whatever stream it writes on
-        v->sync();
-#else
-        v->d_next_level_seed = (int32_t *)malloc((N ? N : 1) * sizeof(int32_t));
-        for (size_t e = 0; e < N; e++) v->d_next_level_seed[e] = -1;
-#endif
-        v->base.next_level_seed = v->d_next_level_seed;
-    }
-    *out = v->d_next_level_seed;
+    v->opt_in_array(v->base.next_level_seed, 1, 0xff);  // every entry -1
+    *out = v->base.next_level_seed;
     return 0;
 }
 
 int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if ((!v->initial_reset_done || !v->base.level_end) && v->capturing())
+    if (!v->begin_opt_in(v->base.level_end != nullptr))
         return -1;
-    v->ensure_initial_reset();
-    if (!v->base.level_end) {
-        const size_t N = (size_t)v->num_envs ? (size_t)v->num_envs : 1;
-        const size_t frames = N * RES_W * RES_H * 3;
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaMalloc((void **)&v->base.final_rgb, frames));
-        CUDA_CHECK(cudaMalloc((void **)&v->base.level_end, N));
-        if (!v->d_reset_list)  // a level bank may have allocated it
-            CUDA_CHECK(cudaMalloc((void **)&v->d_reset_list, N * sizeof(int32_t)));
-        CUDA_CHECK(cudaMemsetAsync(v->base.final_rgb, 0, frames, v->stream));
-        CUDA_CHECK(cudaMemsetAsync(v->base.level_end, 0, N, v->stream));
-        // complete before the caller reads, from whatever stream it reads on
-        v->sync();
-#else
-        v->base.final_rgb = (uint8_t *)calloc(frames, 1);
-        v->base.level_end = (uint8_t *)calloc(N, 1);
-        if (!v->d_reset_list)
-            v->d_reset_list = (int32_t *)calloc(N, sizeof(int32_t));
-#endif
-        v->base.reset_list = v->d_reset_list;
-    }
+    v->opt_in_array(v->base.final_rgb, RES_W * RES_H * 3, 0);
+    v->opt_in_array(v->base.reset_list, 1, 0);
+    v->opt_in_array(v->base.level_end, 1, 0);  // last: a non-null level_end is what selects the two-phase step
     out->rgb = v->base.final_rgb;
     out->level_end = v->base.level_end;
     return 0;
@@ -1141,25 +1141,11 @@ int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *ou
 int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if ((!v->initial_reset_done || !v->d_pause) && v->capturing())
+    if (!v->begin_opt_in(v->d_pause != nullptr))
         return -1;
-    v->ensure_initial_reset();
-    if (!v->d_pause) {
-        const size_t N = (size_t)v->num_envs ? (size_t)v->num_envs : 1;
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaMalloc((void **)&v->d_pause, N));
-        CUDA_CHECK(cudaMalloc((void **)&v->d_paused, N));
-        CUDA_CHECK(cudaMemsetAsync(v->d_pause, 0, N, v->stream));
-        CUDA_CHECK(cudaMemsetAsync(v->d_paused, 0, N, v->stream));
-        // complete before the caller writes, from whatever stream it writes on
-        v->sync();
-#else
-        v->d_pause = (uint8_t *)calloc(N, 1);
-        v->d_paused = (uint8_t *)calloc(N, 1);
-#endif
-        v->base.pause = v->d_pause;
-        v->base.paused = v->d_paused;
-    }
+    v->opt_in_array(v->base.paused, 1, 0);
+    v->opt_in_array(v->d_pause, 1, 0);
+    v->base.pause = v->d_pause;
     *out = v->d_pause;
     return 0;
 }
@@ -1172,27 +1158,23 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
     for (int i = 0; i < count; i++)
         if (seeds[i] < 0)
             return -1;
-    if (v->capturing())
-        return -1;
     std::vector<int32_t> sorted(seeds, seeds + count);
     std::sort(sorted.begin(), sorted.end());
     sorted.erase(std::unique(sorted.begin(), sorted.end()), sorted.end());
     const int n = (int)sorted.size();
     if (v->base.bank.slots ? n > v->bank_capacity : std::max(count, capacity) == 0)
         return -1;  // more distinct seeds than the capacity, or a first call that would fix it at 0
-    v->ensure_initial_reset();
+    if (!v->begin_opt_in(false))  // a build waits for the device, so it never runs under capture
+        return -1;
     KParams &base = v->base;
     const int G = (int)v->games.size();
     if (!base.bank.slots) {
         v->bank_capacity = std::max(count, capacity);
         v->d_bank_seeds = dev_alloc<int32_t>((size_t)v->bank_capacity);
         v->d_bank_count = dev_alloc<int32_t>(1);
-        // a banked step lists its resets as a step with final outputs does (launch_banked_step)
-        base.bank_level_end = dev_alloc<uint8_t>((size_t)v->num_envs);
-        if (!v->d_reset_list) {
-            v->d_reset_list = dev_alloc<int32_t>((size_t)v->num_envs);
-            base.reset_list = v->d_reset_list;
-        }
+        // a banked step lists its resets as a step with final outputs does (launch_step)
+        v->opt_in_array(base.bank_level_end, 1, 0);
+        v->opt_in_array(base.reset_list, 1, 0);
         // per game: int32 usable (16 B) | EnvHdr | Entity[ENT_CAP] | grid[GRID_CAP] | MT19937 | persistent scratch
         size_t total = 0;
         for (const GameVTable *g : v->games) {
@@ -1404,11 +1386,7 @@ uint32_t pgb200_get_errors(libenv_env *handle, uint32_t *host_out) {
     v->sync();
     const size_t N = (size_t)v->num_envs;
     std::vector<EnvHdr> hdr(N);
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(hdr.data(), v->base.hdr, N * sizeof(EnvHdr), cudaMemcpyDeviceToHost));
-#else
-    memcpy(hdr.data(), v->base.hdr, N * sizeof(EnvHdr));
-#endif
+    copy_from_dev(hdr.data(), v->base.hdr, N * sizeof(EnvHdr));
     uint32_t any = 0;
     for (size_t e = 0; e < N; e++) {
         if (host_out)
@@ -1440,32 +1418,16 @@ int pgb200_debug_read_env(libenv_env *handle, int env, void *hdr_out, void *ents
     v->sync();
     EnvHdr hdr;
     const KParams &p = v->base;
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(&hdr, p.hdr + env, sizeof(EnvHdr), cudaMemcpyDeviceToHost));
-#else
-    memcpy(&hdr, p.hdr + env, sizeof(EnvHdr));
-#endif
+    copy_from_dev(&hdr, p.hdr + env, sizeof(EnvHdr));
     if (hdr_out)
         memcpy(hdr_out, &hdr, sizeof(EnvHdr));
     int n = hdr.n_ents < max_ents ? hdr.n_ents : max_ents;
-    if (ents_out && n > 0) {
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaMemcpy(ents_out, p.ents + (size_t)env * p.ent_stride, (size_t)n * sizeof(Entity), cudaMemcpyDeviceToHost));
-#else
-        memcpy(ents_out, p.ents + (size_t)env * p.ent_stride, (size_t)n * sizeof(Entity));
-#endif
-    }
+    if (ents_out && n > 0)
+        copy_from_dev(ents_out, p.ents + (size_t)env * p.ent_stride, (size_t)n * sizeof(Entity));
     return hdr.n_ents;
 }
 
 // ---- get_state / set_state (vecgame.cpp:437-457)
-static void copy_from_dev(void *dst, const void *src, size_t bytes) {
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
-#else
-    memcpy(dst, src, bytes);
-#endif
-}
 
 static void fetch_env(VecEnv *v, int env, host::HostEnv &e) {
     const KParams &p = v->base;

@@ -210,6 +210,12 @@ class BaseProcgenEnv:
         self._keep += [ob_ptrs, ac_ptrs, info_ptrs]
         self._lib.libenv_set_buffers(self._h, C.byref(self._bufs))
 
+    def _alias(self, ptr, shape, typestr):
+        """CUDA tensor aliasing library-owned device memory at `ptr` (an address or a ctypes pointer)."""
+        if not isinstance(ptr, int):
+            ptr = C.cast(ptr, C.c_void_p).value
+        return self._torch.as_tensor(_CudaArray(ptr, shape, typestr), device=self._torch.device("cuda", self.device_index))
+
     def _setup_device_buffers(self):
         torch = self._torch
         if torch is None:
@@ -223,17 +229,13 @@ class BaseProcgenEnv:
             if rc != 0:
                 raise RuntimeError("pgb200_get_device_buffers failed")
             n = self.num
-
-            def alias(ptr, shape, typestr):
-                return torch.as_tensor(_CudaArray(ptr, shape, typestr), device=dev)
-
-            self._rgb = alias(db.rgb, (n, 64, 64, 3), "|u1")
-            self._rew = alias(db.rew, (n,), "<f4")
-            self._first = alias(db.first, (n,), "|u1")
-            self._ac = alias(db.action, (n,), "<i4")
-            self._info = {"prev_level_seed": alias(db.prev_level_seed, (n,), "<i4"),
-                          "prev_level_complete": alias(db.prev_level_complete, (n,), "|u1"),
-                          "level_seed": alias(db.level_seed, (n,), "<i4")}
+            self._rgb = self._alias(db.rgb, (n, 64, 64, 3), "|u1")
+            self._rew = self._alias(db.rew, (n,), "<f4")
+            self._first = self._alias(db.first, (n,), "|u1")
+            self._ac = self._alias(db.action, (n,), "<i4")
+            self._info = {"prev_level_seed": self._alias(db.prev_level_seed, (n,), "<i4"),
+                          "prev_level_complete": self._alias(db.prev_level_complete, (n,), "|u1"),
+                          "level_seed": self._alias(db.level_seed, (n,), "<i4")}
         self._dev = dev
         self._pinned_ac = None
 
@@ -366,8 +368,7 @@ class BaseProcgenEnv:
             with torch.cuda.device(self.device_index):
                 if self._lib.pgb200_get_next_level_seeds(self._h, C.byref(ptr)) != 0:
                     raise RuntimeError("pgb200_get_next_level_seeds failed")
-                dev = torch.device("cuda", self.device_index)
-                self._next_level_seeds = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "<i4"), device=dev)
+                self._next_level_seeds = self._alias(ptr, (self.num,), "<i4")
         return self._next_level_seeds
 
     def final_outputs(self):
@@ -389,11 +390,8 @@ class BaseProcgenEnv:
             with torch.cuda.device(self.device_index):
                 if self._lib.pgb200_get_final_outputs(self._h, C.byref(out)) != 0:
                     raise RuntimeError("pgb200_get_final_outputs failed")
-                dev = torch.device("cuda", self.device_index)
-                self._final_outputs = {
-                    "rgb": torch.as_tensor(_CudaArray(out.rgb, (self.num, 64, 64, 3), "|u1"), device=dev),
-                    "level_end": torch.as_tensor(_CudaArray(out.level_end, (self.num,), "|u1"), device=dev),
-                }
+                self._final_outputs = {"rgb": self._alias(out.rgb, (self.num, 64, 64, 3), "|u1"),
+                                       "level_end": self._alias(out.level_end, (self.num,), "|u1")}
         return dict(self._final_outputs)
 
     def pause_mask(self):
@@ -418,8 +416,7 @@ class BaseProcgenEnv:
             with torch.cuda.device(self.device_index):
                 if self._lib.pgb200_get_pause_mask(self._h, C.byref(ptr)) != 0:
                     raise RuntimeError("pgb200_get_pause_mask failed")
-                dev = torch.device("cuda", self.device_index)
-                self._pause_mask = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (self.num,), "|u1"), device=dev)
+                self._pause_mask = self._alias(ptr, (self.num,), "|u1")
         return self._pause_mask
 
     def build_level_bank(self, seeds=None, capacity: int = 0) -> None:
@@ -649,11 +646,10 @@ class BaseProcgenEnv:
         (consumer_observation() does the same once the handle has been captured.) Written on the stream the
         handle steps on."""
         if self._consumer_slot is None:
-            torch = self._torch
             ptr = C.POINTER(C.c_int32)()
             if self._lib.pgb200_get_consumer_slot_device(self._h, C.byref(ptr)) != 0:
                 raise RuntimeError("pgb200_get_consumer_slot_device failed")
-            self._consumer_slot = torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (1,), "<i4"), device=self._dev)
+            self._consumer_slot = self._alias(ptr, (1,), "<i4")
         return self._consumer_slot
 
     def consumer_ring(self):

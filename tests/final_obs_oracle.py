@@ -17,8 +17,8 @@ import os
 
 import numpy as np
 
-from helpers import assert_same_observation
-from level_seed_oracle import emulate_step, next_level_seeds, read_seeds, write_seeds
+from helpers import assert_same_observation, lib_array, read_lib_array, write_lib_array
+from level_seed_oracle import emulate_step, next_level_seeds
 from oracle.record import STANDIN_PACK, oracle_env, recording_dir, use_records
 from oracle.ref_env import REF_LIB, RefVecEnv, mt19937_actions
 
@@ -98,31 +98,16 @@ class LibFinal:
         lib = env.lib
         lib.pgb200_get_final_outputs.argtypes = [C.c_void_p, C.POINTER(FinalOutputs)]
         lib.pgb200_get_final_outputs.restype = C.c_int
-        lib.pgb200_is_device_build.restype = C.c_int
         out = FinalOutputs()
         assert lib.pgb200_get_final_outputs(C.c_void_p(env.h), C.byref(out)) == 0
-        n = env.num
-        if not lib.pgb200_is_device_build():
-            self._rgb = np.ctypeslib.as_array(C.cast(out.rgb, C.POINTER(C.c_uint8)), shape=(n,) + FRAME)
-            self._level_end = np.ctypeslib.as_array(C.cast(out.level_end, C.POINTER(C.c_uint8)), shape=(n,))
-        else:
-            import torch
-
-            from procgen_b200.env import _CudaArray
-
-            self._rgb = torch.as_tensor(_CudaArray(out.rgb, (n,) + FRAME, "|u1"), device="cuda")
-            self._level_end = torch.as_tensor(_CudaArray(out.level_end, (n,), "|u1"), device="cuda")
+        self._rgb = lib_array(env, out.rgb, (env.num,) + FRAME, "|u1")
+        self._level_end = lib_array(env, out.level_end, (env.num,), "|u1")
 
     def prepare(self, actions):
         pass
 
     def read(self):
-        if isinstance(self._rgb, np.ndarray):
-            return self._level_end.copy(), self._rgb.copy()
-        import torch
-
-        torch.cuda.synchronize()
-        return self._level_end.cpu().numpy(), self._rgb.cpu().numpy()
+        return read_lib_array(self._level_end), read_lib_array(self._rgb)
 
     def close(self):
         pass
@@ -178,7 +163,7 @@ def run_final_lockstep(ref, ref_fin, dut, steps, plan=None, overrides=False, act
         if overrides:
             for e, s in new.items():
                 pending[e] = s
-            write_seeds(seeds, pending)
+            write_lib_array(seeds, pending)
         if t % blob_every == 0:
             for e in range(n):
                 assert ref.get_state(e) == dut.get_state(e), f"step {t} env {e}: state blobs differ"
@@ -207,7 +192,7 @@ def run_final_lockstep(ref, ref_fin, dut, steps, plan=None, overrides=False, act
         assert ok.all(), f"step {t}: level_end {le_d[~ok][:8]} where first is {dut.first[~ok][:8]} (envs {np.nonzero(~ok)[0][:8]})"
         if overrides:
             pending[took] = -1
-            assert np.array_equal(read_seeds(seeds), pending), f"step {t}: override array"
+            assert np.array_equal(read_lib_array(seeds), pending), f"step {t}: override array"
         dut_rgb = rgb_d
         ends[t] = le_d
     for e in range(n):

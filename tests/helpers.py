@@ -1,4 +1,5 @@
 """Shared test helpers: lockstep comparison of any libenv-ABI implementation against the oracle."""
+import ctypes as C
 import os
 
 import numpy as np
@@ -23,6 +24,44 @@ def make_checked_pair(lib_path, num, env_name, extra_options=None, launch_shape=
     dut = RefVecEnv(num, env_name, lib_path=lib_path, resource_root=STANDIN_PACK, extra_options=extra_options,
                     launch_shape=launch_shape, ob_layout=ob_layout, **kw)
     return ref, dut
+
+
+def lib_array(env, ptr, shape, typestr):
+    """An array the library under test hands out for a libenv-ABI env (oracle.ref_env.RefVecEnv), at `ptr` (an
+    address or a ctypes pointer): a numpy view in the host debug build, a torch CUDA tensor aliasing device memory
+    in the GPU build."""
+    env.lib.pgb200_is_device_build.restype = C.c_int
+    addr = ptr if isinstance(ptr, int) else C.cast(ptr, C.c_void_p).value
+    if not env.lib.pgb200_is_device_build():
+        ctype = np.ctypeslib.as_ctypes_type(np.dtype(typestr))
+        return np.ctypeslib.as_array(C.cast(addr, C.POINTER(ctype)), shape=shape)
+    import torch
+
+    from procgen_b200.env import _CudaArray
+
+    return torch.as_tensor(_CudaArray(addr, shape, typestr), device="cuda")
+
+
+def write_lib_array(arr, values):
+    """Write the whole of a lib_array; a device array is written with torch and synchronised (libenv_act needs the
+    writes complete before it is called)."""
+    if isinstance(arr, np.ndarray):
+        arr[:] = values
+        return
+    import torch
+
+    arr.copy_(torch.as_tensor(np.asarray(values)).to(arr.device))
+    torch.cuda.synchronize()
+
+
+def read_lib_array(arr):
+    """A host copy of a lib_array, once the device's work so far is complete."""
+    if isinstance(arr, np.ndarray):
+        return arr.copy()
+    import torch
+
+    torch.cuda.synchronize()
+    return arr.cpu().numpy()
 
 
 def assert_same_observation(ref, dut, t, rgb_tol=0):

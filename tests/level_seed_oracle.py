@@ -12,6 +12,7 @@ import struct
 
 import numpy as np
 
+from helpers import lib_array, read_lib_array, write_lib_array
 from oracle.state_blob import Reader, parse
 
 # The oracle's recorded outputs of tests/test_gpu_level_seeds.py, kept apart from tests/golden/oracle_records.json.gz
@@ -71,37 +72,14 @@ def patch_fields(blob, **fields):
 
 
 def next_level_seeds(env):
-    """The override array of a libenv-ABI env of the library under test (oracle.ref_env.RefVecEnv): a numpy
-    view in the host debug build, an int32 torch CUDA tensor aliasing device memory in the GPU build."""
+    """The int32 override array of a libenv-ABI env of the library under test (oracle.ref_env.RefVecEnv), as
+    helpers.lib_array."""
     lib = env.lib
     lib.pgb200_get_next_level_seeds.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
     lib.pgb200_get_next_level_seeds.restype = C.c_int
-    lib.pgb200_is_device_build.restype = C.c_int
     ptr = C.POINTER(C.c_int32)()
     assert lib.pgb200_get_next_level_seeds(C.c_void_p(env.h), C.byref(ptr)) == 0
-    if not lib.pgb200_is_device_build():
-        return np.ctypeslib.as_array(ptr, shape=(env.num,))
-    import torch
-
-    from procgen_b200.env import _CudaArray
-
-    return torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (env.num,), "<i4"), device="cuda")
-
-
-def write_seeds(seeds, values):
-    """Write the whole override array; a device array is written with torch and synchronised (libenv_act
-    needs the writes complete before it is called)."""
-    if isinstance(seeds, np.ndarray):
-        seeds[:] = values
-        return
-    import torch
-
-    seeds.copy_(torch.as_tensor(np.asarray(values, np.int32)).to(seeds.device))
-    torch.cuda.synchronize()
-
-
-def read_seeds(seeds):
-    return np.array(seeds, np.int64) if isinstance(seeds, np.ndarray) else seeds.cpu().numpy().astype(np.int64)
+    return lib_array(env, ptr, (env.num,), "<i4")
 
 
 def emulate_step(ref, actions, overrides):
@@ -150,7 +128,7 @@ def run_override_lockstep(ref, dut, steps, plan, action_seed=0):
 
     n = ref.num
     seeds = next_level_seeds(dut)
-    pending = read_seeds(seeds)
+    pending = read_lib_array(seeds).astype(np.int64)
     assert (pending == -1).all(), "a new override array holds -1 everywhere"
     acts = mt19937_actions(action_seed, n, steps)
     assert_same_observation(ref, dut, -1)
@@ -159,7 +137,7 @@ def run_override_lockstep(ref, dut, steps, plan, action_seed=0):
         a = acts[t].copy()
         for e, s in plan(t, a, pending.copy()).items():
             pending[e] = s
-        write_seeds(seeds, pending)
+        write_lib_array(seeds, pending)
         dut_pre = [dut.get_state(e) for e in range(n)]
         pre, took = emulate_step(ref, a, pending)
         for e in range(n):
@@ -169,7 +147,7 @@ def run_override_lockstep(ref, dut, steps, plan, action_seed=0):
         for e in took:
             assert dut.info["level_seed"][e] == pending[e], f"step {t} env {e}: override not played"
         pending[took] = -1
-        now = read_seeds(seeds)
+        now = read_lib_array(seeds)
         assert np.array_equal(now, pending), f"step {t}: override array {now[now != pending][:8]} where {pending[now != pending][:8]} was expected"
         taken += len(took)
     for e in range(n):
@@ -201,18 +179,18 @@ def check_consumed_kept_and_set_state(lib_path, resource_root=None):
     donor = RefVecEnv(8, "coinrun", rand_seed=7, **kw)
     seeds = next_level_seeds(dut)
     want = np.array([100, 101, 102, 103, 104, 105, 106, -1])
-    write_seeds(seeds, want)
+    write_lib_array(seeds, want)
     for e in range(8):
         dut.set_state(e, donor.get_state(e))
-    assert np.array_equal(read_seeds(seeds), want)
+    assert np.array_equal(read_lib_array(seeds), want)
     for e in range(8):
         assert dut.get_state(e) == donor.get_state(e), "get_state carries no override"
     acts = np.array([-1, -1, -1, -1, 4, 4, 4, -1], np.int32)
     dut.act(acts)
     dut.observe()
-    got = read_seeds(seeds)
+    got = read_lib_array(seeds)
     assert np.array_equal(got[:4], [-1] * 4) and np.array_equal(got[4:], want[4:])
     assert np.array_equal(dut.info["level_seed"][:4], want[:4])
-    assert dut.first[7] == 1 and read_seeds(seeds)[7] == -1
+    assert dut.first[7] == 1 and read_lib_array(seeds)[7] == -1
     dut.close()
     donor.close()

@@ -12,8 +12,8 @@ import zlib
 
 import numpy as np
 
-from helpers import assert_same_observation
-from level_seed_oracle import emulate_step, next_level_seeds, read_seeds, write_seeds
+from helpers import assert_same_observation, read_lib_array, write_lib_array
+from level_seed_oracle import emulate_step, next_level_seeds
 from oracle.ref_env import mt19937_actions
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -83,20 +83,20 @@ def run_level_sweep(ref, dut, seeds, rollout, action_seed=0):
     error bits must stay 0. Returns the number of batches."""
     n = dut.num
     arr = next_level_seeds(dut)
-    assert (read_seeds(arr) == -1).all(), "a new override array holds -1 everywhere"
+    assert (read_lib_array(arr) == -1).all(), "a new override array holds -1 everywhere"
     force = np.full(n, -1, np.int32)
     assert_same_observation(ref, dut, "initial reset")
     batches = 0
     for b in range(0, len(seeds), n):
         batch = np.resize(np.asarray(seeds[b:b + n], np.int64), n)
         label = f"seeds {b}..{b + n - 1} ({batch[0]}, ...)"
-        write_seeds(arr, batch)
+        write_lib_array(arr, batch)
         _, took = emulate_step(ref, force, batch)
         assert took == list(range(n)), f"{label}: the reference did not reset every env"
         dut.act(force)
         assert_same_observation(ref, dut, label)
         assert np.array_equal(dut.info["level_seed"], batch), f"{label}: info level_seed is not the chosen seeds"
-        assert (read_seeds(arr) == -1).all(), f"{label}: the override array was not consumed"
+        assert (read_lib_array(arr) == -1).all(), f"{label}: the override array was not consumed"
         assert_same_blobs(ref, dut, f"{label}, generated:")
         acts = mt19937_actions(action_seed + batches, n, rollout)
         for t in range(rollout):
@@ -124,7 +124,7 @@ def run_sequential_wrap(ref, dut, steps, action_seed=0):
     seeds = np.array(sequential_wrap_seeds(n), np.int64)
     force = np.full(n, -1, np.int32)
     assert_same_observation(ref, dut, "initial reset")
-    write_seeds(arr, seeds)
+    write_lib_array(arr, seeds)
     emulate_step(ref, force, seeds)
     dut.act(force)
     assert_same_observation(ref, dut, "overrides")

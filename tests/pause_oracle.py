@@ -15,7 +15,8 @@ import os
 
 import numpy as np
 
-from level_seed_oracle import emulate_step, next_level_seeds, read_seeds, write_seeds
+from helpers import lib_array, read_lib_array, write_lib_array
+from level_seed_oracle import emulate_step, next_level_seeds
 from oracle.ref_env import mt19937_actions
 
 PAUSE_RECORDS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pause_records.json.gz")
@@ -29,38 +30,14 @@ def use_pause_records():
 
 
 def pause_mask(env):
-    """The pause mask of a libenv-ABI env of the library under test (oracle.ref_env.RefVecEnv): a numpy view in
-    the host debug build, a uint8 torch CUDA tensor aliasing device memory in the GPU build."""
+    """The uint8 pause mask of a libenv-ABI env of the library under test (oracle.ref_env.RefVecEnv), as
+    helpers.lib_array."""
     lib = env.lib
     lib.pgb200_get_pause_mask.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8))]
     lib.pgb200_get_pause_mask.restype = C.c_int
-    lib.pgb200_is_device_build.restype = C.c_int
     ptr = C.POINTER(C.c_uint8)()
     assert lib.pgb200_get_pause_mask(C.c_void_p(env.h), C.byref(ptr)) == 0
-    if not lib.pgb200_is_device_build():
-        return np.ctypeslib.as_array(ptr, shape=(env.num,))
-    import torch
-
-    from procgen_b200.env import _CudaArray
-
-    return torch.as_tensor(_CudaArray(C.cast(ptr, C.c_void_p).value, (env.num,), "|u1"), device="cuda")
-
-
-def write_mask(mask, paused):
-    """Write the whole mask; a device mask is written with torch and synchronised (libenv_act needs the writes
-    complete before it is called)."""
-    values = np.asarray(paused, np.uint8)
-    if isinstance(mask, np.ndarray):
-        mask[:] = values
-        return
-    import torch
-
-    mask.copy_(torch.as_tensor(values).to(mask.device))
-    torch.cuda.synchronize()
-
-
-def read_mask(mask):
-    return np.array(mask, np.uint8) if isinstance(mask, np.ndarray) else mask.cpu().numpy()
+    return lib_array(env, ptr, (env.num,), "|u1")
 
 
 def emulate_pause_step(ref, actions, paused, overrides=None):
@@ -169,7 +146,7 @@ def run_pause_lockstep(ref, dut, steps, pause_plan, plan=None, overrides=False, 
 
     n = ref.num
     mask = pause_mask(dut)
-    assert not read_mask(mask).any(), "a new pause mask holds 0 everywhere"
+    assert not read_lib_array(mask).any(), "a new pause mask holds 0 everywhere"
     seeds = next_level_seeds(dut) if overrides else None
     dut_fin = LibFinal(dut) if final is not None else None
     checked = hasattr(ref, "_fold")
@@ -188,11 +165,11 @@ def run_pause_lockstep(ref, dut, steps, pause_plan, plan=None, overrides=False, 
         new = plan(t, a, pending.copy()) if plan else {}
         if force_paused:
             a[paused] = -1
-        write_mask(mask, paused)
+        write_lib_array(mask, paused)
         if overrides:
             for e, s in new.items():
                 pending[e] = s
-            write_seeds(seeds, pending)
+            write_lib_array(seeds, pending)
         if final is not None:
             final.prepare(a)
         pre, took = emulate_pause_step(ref, a, paused, pending if overrides else None)
@@ -216,8 +193,8 @@ def run_pause_lockstep(ref, dut, steps, pause_plan, plan=None, overrides=False, 
         if overrides:
             assert not paused[took].any()
             pending[took] = -1
-            assert np.array_equal(read_seeds(seeds), pending), f"step {t}: override array"
-        assert np.array_equal(read_mask(mask), paused.astype(np.uint8)), f"step {t}: the step changed the mask"
+            assert np.array_equal(read_lib_array(seeds), pending), f"step {t}: override array"
+        assert np.array_equal(read_lib_array(mask), paused.astype(np.uint8)), f"step {t}: the step changed the mask"
         hist[t] = paused
     for e in range(n):
         assert ref.get_state(e) == dut.get_state(e), f"env {e}: state blobs differ at the end"
@@ -234,7 +211,7 @@ def check_set_state_into_paused_env(ref, dut, steps=30):
     mask = pause_mask(dut)
     paused = np.zeros(n, bool)
     paused[::2] = True
-    write_mask(mask, paused)
+    write_lib_array(mask, paused)
     acts = mt19937_actions(3, n, steps)
     for t in range(steps):
         ref.act(acts[t])
@@ -242,7 +219,7 @@ def check_set_state_into_paused_env(ref, dut, steps=30):
     donor = [ref.get_state(e) for e in range(n)]
     for e in np.nonzero(paused)[0]:
         dut.set_state(int(e), donor[e])
-    assert np.array_equal(read_mask(mask), paused.astype(np.uint8)), "set_state changed the mask"
+    assert np.array_equal(read_lib_array(mask), paused.astype(np.uint8)), "set_state changed the mask"
     _, ob, _ = dut.observe()
     r_ob = ref.observe()[1]["rgb"]
     assert np.array_equal(ob["rgb"][paused], r_ob[paused]), "set_state did not render the loaded state"

@@ -11,8 +11,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import make_checked_pair, run_lockstep
-from level_seed_oracle import (check_consumed_kept_and_set_state, emulate_step, read_seeds, refill_plan, run_override_lockstep,
+from helpers import make_checked_pair, read_lib_array, run_lockstep
+from level_seed_oracle import (check_consumed_kept_and_set_state, emulate_step, refill_plan, run_override_lockstep,
                                use_level_seed_records)
 from oracle.record import STANDIN_PACK, oracle_env
 from oracle.ref_env import MAX_STATE_SIZE, mt19937_actions
@@ -82,7 +82,7 @@ def test_array_requested_but_unused_changes_nothing(product_lib):
                                  num_levels=200, start_level=0, rand_seed=0)
     seeds = next_level_seeds(dut)
     run_lockstep(ref, dut, 500)
-    assert (read_seeds(seeds) == -1).all()
+    assert (read_lib_array(seeds) == -1).all()
     ref.close()
     dut.close()
 
@@ -209,7 +209,7 @@ def test_host_buffers_python_accessor(product_lib):
         for k in ("prev_level_seed", "prev_level_complete", "level_seed"):
             assert np.array_equal(env._info[k], ref.info[k]), f"step {t}: info[{k}]"
         pending[took] = -1
-        assert np.array_equal(read_seeds(seeds), pending), f"step {t}: override array"
+        assert np.array_equal(read_lib_array(seeds), pending), f"step {t}: override array"
     assert env.errors() == 0
     env.close()
     ref.close()

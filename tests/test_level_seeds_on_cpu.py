@@ -4,9 +4,9 @@ level_seed_oracle.py), state blobs included, and the override array is consumed 
 import numpy as np
 import pytest
 
-from helpers import make_pair, run_lockstep
+from helpers import make_pair, read_lib_array, run_lockstep, write_lib_array
 from level_seed_oracle import (check_consumed_kept_and_set_state, emulate_step, field_offsets, next_level_seeds, patch_fields,
-                               read_seeds, refill_plan, run_override_lockstep, write_seeds)
+                               refill_plan, run_override_lockstep)
 from oracle.state_blob import parse
 
 ALL16 = "bigfish,bossfight,caveflyer,chaser,climber,coinrun,dodgeball,fruitbot,heist,jumper,leaper,maze,miner,ninja,plunder,starpilot"
@@ -71,9 +71,9 @@ def test_sequential_levels_continue_from_override(ref_lib, hostsim_lib):
     ref, dut = make_pair(hostsim_lib, 8, "maze", distribution_mode="easy", num_levels=3, start_level=0, rand_seed=0,
                          use_sequential_levels=True)
     seeds = next_level_seeds(dut)
-    write_seeds(seeds, np.arange(8) + 4000)
+    write_lib_array(seeds, np.arange(8) + 4000)
     acts = np.full(8, -1, np.int32)
-    pre, took = emulate_step(ref, acts, read_seeds(seeds))
+    pre, took = emulate_step(ref, acts, read_lib_array(seeds))
     dut.act(acts)
     assert took == list(range(8))
     from helpers import assert_same_observation
@@ -99,7 +99,7 @@ def test_array_requested_but_unused_changes_nothing(ref_lib, hostsim_lib):
     ref, dut = make_pair(hostsim_lib, 16, ALL16, launch_shape=(3, False), **KW)
     seeds = next_level_seeds(dut)
     run_lockstep(ref, dut, 200)
-    assert (read_seeds(seeds) == -1).all()
+    assert (read_lib_array(seeds) == -1).all()
     ref.close()
     dut.close()
 
