@@ -16,7 +16,7 @@ struct KParams {
     int32_t *scratch;
     RotBlit *rot_scratch;       // [N][rot_stride] rotated-sprite / span records
     Blit *blit_list;            // [N][blit_stride] background-less blit lists (entities in draw order, then overlays)
-    unsigned char *frame_setup; // [N][frame_setup_stride bytes] FrameSetupT of the env's game
+    unsigned char *frame_setup; // [N][frame_setup_stride bytes] FrameSharedT of the env's game (setup kernel -> render kernel)
     Blit *cell_spill;           // [N][cell_spill_stride] general cell blits that do not fit the render CTA's shared memory
     const GameAssets *assets;   // table of the game this launch handles
     const uint32_t *atlas;
@@ -293,16 +293,39 @@ PG_HD void bank_generate_level(const KParams &p, int item, unsigned char *stage)
     *reinterpret_cast<int32_t *>(slot) = usable ? 1 : 0;  // every lane stores the same value
 }
 
+// Profiling variant (-DPG_PHASE_TIMING): the setup kernel's phases, SM cycles of env's last frame in header slots
+// the render kernel does not write (it takes 0, 5, 6, 7): 1 setup_frame, 2 entity blits (with the tiles and
+// rotated sprites they reserved, and the overlays), 3 frame_build, 4 frame_tile_alloc, 8 frame_cells_finish,
+// 9 the store of the record. A reset earlier in the same step leaves level-generation cycles in these slots;
+// the setup kernel overwrites them.
+#if defined(PG_PHASE_TIMING) && defined(__CUDA_ARCH__)
+#define PG_SETUP_PHASE_BEGIN long long _pg_s0 = clock64()
+#define PG_SETUP_PHASE(id)                                    \
+    do {                                                      \
+        const long long _pg_s1 = clock64();                   \
+        if (lane == 0)                                        \
+            p.hdr[env].dbg_phase[id] = (uint32_t)(_pg_s1 - _pg_s0); \
+        _pg_s0 = _pg_s1;                                      \
+    } while (0)
+#else
+#define PG_SETUP_PHASE_BEGIN do { } while (0)
+#define PG_SETUP_PHASE(id) do { } while (0)
+#endif
+
 // ---- setup kernel body: one warp (lanes `lane` of `nlanes`) prepares everything about env's frame that
-// does not depend on pixels or cells: camera, spans, background / overlay / entity blits
+// does not depend on pixels or cells: camera, spans, background / overlay / entity blits. `f` is the warp's
+// own record (shared memory on the device), which holds whatever the warp's previous env left in it: every
+// field is written for this frame before it is read.
 template <class G, class Setup>
 PG_HD void env_setup_frame(const KParams &p, int env, Setup &f, int lane, int nlanes) {
+    PG_SETUP_PHASE_BEGIN;
     Ctx c = make_ctx(p, env);
     using R = Raster<G, Setup>;
     R::setup_frame(c, f, p.snap != 0, lane, nlanes);
 #if defined(__CUDA_ARCH__)
     __syncwarp();
 #endif
+    PG_SETUP_PHASE(1);
     R::build_entity_blits(c, f, lane, nlanes);
 #if defined(__CUDA_ARCH__)
     __syncwarp();
@@ -327,18 +350,36 @@ PG_HD void env_setup_frame(const KParams &p, int env, Setup &f, int lane, int nl
 #if defined(__CUDA_ARCH__)
         __syncwarp();
 #endif
+        PG_SETUP_PHASE(2);
         R::frame_build(c, f, lane, nlanes, 0);
 #if defined(__CUDA_ARCH__)
         __syncwarp();
 #endif
+        PG_SETUP_PHASE(3);
         R::frame_tile_alloc(c, f, p.tiles, lane, nlanes);
 #if defined(__CUDA_ARCH__)
         __syncwarp();
 #endif
+        PG_SETUP_PHASE(4);
         R::frame_cells_finish(c, f, lane, nlanes);
+        PG_SETUP_PHASE(8);
     } else {
+        PG_SETUP_PHASE(2);
         R::frame_build(c, f, lane, nlanes, 0);  // background row offsets only
+        PG_SETUP_PHASE(3);
+        PG_SETUP_PHASE(4);
+        PG_SETUP_PHASE(8);
     }
+}
+
+// The setup kernel's result, the FrameSharedT prefix of the warp's record `f`, stored to env's slot of
+// p.frame_setup with 16-byte vectors, the warp's lanes side by side (one lane in the host debug build). The render
+// kernel stages it from there. The rest of the record is the setup kernel's own scratch and stays where it is.
+template <class Setup>
+PG_HD void env_store_frame(const KParams &p, int env, const Setup &f) {
+    using Shared = typename Setup::Shared;
+    static_assert(sizeof(Shared) % 16 == 0, "the record is stored in 16-byte vectors");
+    bank_copy_vecs(p.frame_setup + (size_t)env * p.frame_setup_stride, static_cast<const Shared *>(&f), (int)sizeof(Shared));
 }
 
 // Host debug harness twin of the bulk copies that stage the frame's tiles

@@ -142,22 +142,40 @@ __global__ void __launch_bounds__(kLogicThreads) bank_build_kernel(KParams p, un
 // entity blits (incl. the scan conversion of rotated sprites). Every warp of the grid runs this
 // same code, which is what the instruction cache wants; the render kernel that follows — one CTA
 // per env — is left with the O(pixels + cells) work and picks the result up with one bulk copy.
+// Each warp builds its env's FrameSetupT in its own slot of the block's shared memory — the record's
+// counters are shared-memory atomics and its read-backs shared-memory loads — and stores the FrameSharedT
+// prefix to the env's global record once, at the end.
 constexpr int kSetupThreads = 128;
 #ifndef PG_SETUP_MIN_BLOCKS
 #define PG_SETUP_MIN_BLOCKS 8   // 64 registers x 32 warps/SM: more envs in flight beat more registers (96 x 20 was slower)
 #endif
+// Resident setup blocks per SM: PG_SETUP_MIN_BLOCKS, or as many as the warps' records (shared memory) allow;
+// the register cap follows (65536 / (128 * blocks)).
+template <class G, int VIEW>
+struct SetupTune {
+    static constexpr int kSmemBytes = (int)sizeof(typename FrameFor<G, VIEW>::setup) * (kSetupThreads / 32);
+    // 227 KiB usable per SM, 1 KiB reserved per resident CTA, 128 B of static shared memory (build_entity_blits)
+    static constexpr int kFit = (227 * 1024) / (kSmemBytes + 1024 + 128);
+    static constexpr int kMinBlocks = kFit >= PG_SETUP_MIN_BLOCKS ? PG_SETUP_MIN_BLOCKS : (kFit >= 1 ? kFit : 1);
+};
 // LIST: phase B of a step with final outputs, the warps of the grid stride over p.reset_list (which never holds a
 // paused env). PAUSE: a paused env's warp returns; its frame_setup slot goes stale, and nothing reads it.
 template <class G, int VIEW, bool LIST = false, bool PAUSE = false>
-__global__ void __launch_bounds__(kSetupThreads, PG_SETUP_MIN_BLOCKS) setup_kernel(KParams p) {
+__global__ void __launch_bounds__(kSetupThreads, SetupTune<G, VIEW>::kMinBlocks) setup_kernel(KParams p) {
     using Setup = typename FrameFor<G, VIEW>::setup;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    Setup &f = reinterpret_cast<Setup *>(smem_raw)[threadIdx.x >> 5];
+    const int lane = (int)(threadIdx.x & 31u);
     const int i = (int)blockIdx.x * (kSetupThreads / 32) + (int)(threadIdx.x >> 5);
     if (LIST) {
         const int count = (int)*p.reset_count;
         for (int j = i; j < count; j += (int)gridDim.x * (kSetupThreads / 32)) {
             const int env = p.reset_list[j];
-            Setup &f = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
-            env_setup_frame<G, Setup>(p, env, f, (int)(threadIdx.x & 31u), 32);
+            env_setup_frame<G, Setup>(p, env, f, lane, 32);
+            __syncwarp();
+            PG_SETUP_PHASE_BEGIN;
+            env_store_frame<Setup>(p, env, f);  // ends with a __syncwarp: the next env may reuse the slot
+            PG_SETUP_PHASE(9);
         }
         return;
     }
@@ -166,8 +184,11 @@ __global__ void __launch_bounds__(kSetupThreads, PG_SETUP_MIN_BLOCKS) setup_kern
     const int env = p.env_first + i * p.env_step;
     if (PAUSE && p.paused[env])
         return;
-    Setup &f = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
-    env_setup_frame<G, Setup>(p, env, f, (int)(threadIdx.x & 31u), 32);
+    env_setup_frame<G, Setup>(p, env, f, lane, 32);
+    __syncwarp();
+    PG_SETUP_PHASE_BEGIN;
+    env_store_frame<Setup>(p, env, f);
+    PG_SETUP_PHASE(9);
 }
 
 #ifndef PG_RENDER_CTAS_PER_SM
@@ -253,8 +274,7 @@ __device__ __forceinline__ void render_env_frame(const KParams &p, typename Fram
 #define PG_RENDER_PHASE(id) do { } while (0)
 #endif
     using Shared = typename FrameFor<G, VIEW>::shared;
-    using Setup = typename FrameFor<G, VIEW>::setup;
-    const Setup *gs = reinterpret_cast<const Setup *>(p.frame_setup + (size_t)env_of() * p.frame_setup_stride);
+    const Shared *gs = reinterpret_cast<const Shared *>(p.frame_setup + (size_t)env_of() * p.frame_setup_stride);
     if (tid < 32) {
         // Everything the setup kernel prepared for this env — one bulk copy into the head of the frame —
         // and the pre-scaled tiles its cells need, one bulk copy each, all counted on one mbarrier phase.
@@ -264,7 +284,7 @@ __device__ __forceinline__ void render_env_frame(const KParams &p, typename Fram
         for (int d = 16; d > 0; d >>= 1) words += __shfl_xor_sync(0xffffffffu, words, d);
         if (tid == 0) {
             pg_mbar_arrive_expect_tx(&f.mbar, (unsigned)sizeof(Shared) + 4u * words);
-            pg_bulk_load(static_cast<Shared *>(&f), static_cast<const Shared *>(gs), (unsigned)sizeof(Shared), &f.mbar);
+            pg_bulk_load(static_cast<Shared *>(&f), gs, (unsigned)sizeof(Shared), &f.mbar);
         }
         __syncwarp();
         for (int j = tid; j < nj; j += 32)
@@ -408,9 +428,14 @@ void render_env_serial(const KParams &p, int env) {
     using Setup = typename FrameFor<G, VIEW>::setup;
     using Shared = typename FrameFor<G, VIEW>::shared;
     static thread_local Frame *f = new Frame;
-    Setup &s = *reinterpret_cast<Setup *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
-    env_setup_frame<G, Setup>(p, env, s, 0, 1);
-    static_cast<Shared &>(*f) = static_cast<const Shared &>(s);
+    static thread_local Setup *s = new Setup;
+    // The device's record is a shared-memory slot that holds whatever its warp's previous env left in it. Here it is
+    // poisoned before every frame, so that the parity suites fail if setup reads a field it has not written for this
+    // frame, or if the render path depends on a stored byte that setup left unwritten.
+    memset(static_cast<void *>(s), 0xA5, sizeof(Setup));
+    env_setup_frame<G, Setup>(p, env, *s, 0, 1);
+    env_store_frame<Setup>(p, env, *s);
+    static_cast<Shared &>(*f) = *reinterpret_cast<const Shared *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
     env_stage_tiles_serial<Frame>(p, *f);
     for (int w = 0; w < 4; w++) env_render_compose<G, Frame>(p, *f, w, 4, 0, 1);  // the device's row ownership, one lane per owner
     uint8_t *rgb = PASS == 1 && p.level_end[env] != 0 ? p.final_rgb : p.rgb;
@@ -449,6 +474,21 @@ int prepare_render_smem(const LaunchCtx &lc) {
     if (have < bytes) {
         CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS, PAUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
         have = bytes;
+    }
+    return bytes;
+}
+
+// Dynamic shared memory of one setup block (one FrameSetupT per warp) with the kernel's opt-in limit raised to it
+// once (needed above 48 KiB: the whole-world views)
+template <class G, int VIEW, bool LIST, bool PAUSE>
+int prepare_setup_smem() {
+    constexpr int bytes = SetupTune<G, VIEW>::kSmemBytes;
+    static bool attr_set[64] = {};
+    int dev = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    if (!attr_set[dev & 63]) {
+        CUDA_CHECK(cudaFuncSetAttribute(setup_kernel<G, VIEW, LIST, PAUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        attr_set[dev & 63] = true;
     }
     return bytes;
 }
@@ -520,17 +560,18 @@ template <class G, int VIEW, int PASS, bool PAUSE>
 void frames_phase(const KParams &p, const LaunchCtx &lc) {
     constexpr bool LIST = PASS == 2;
 #ifndef PG_HOSTSIM
+    const int setup_smem = prepare_setup_smem<G, VIEW, LIST, PAUSE>();
     const int render_smem = prepare_render_smem<G, VIEW, PASS, PAUSE>(lc);
     int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
     int render_blocks = p.env_count;
     if (LIST) {
-        const int setup_fit = lc.num_sms * PG_SETUP_MIN_BLOCKS, render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
+        const int setup_fit = lc.num_sms * SetupTune<G, VIEW>::kMinBlocks, render_fit = lc.num_sms * RenderTune<G, VIEW>::kMinBlocks;
         setup_blocks = setup_blocks < setup_fit ? setup_blocks : setup_fit;
         render_blocks = render_blocks < render_fit ? render_blocks : render_fit;
     }
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[1], lc.stream));
-    setup_kernel<G, VIEW, LIST, PAUSE><<<setup_blocks, kSetupThreads, 0, lc.stream>>>(p);
+    setup_kernel<G, VIEW, LIST, PAUSE><<<setup_blocks, kSetupThreads, setup_smem, lc.stream>>>(p);
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
     render_kernel<G, VIEW, PASS, PAUSE><<<render_blocks, kRenderThreads, render_smem, lc.stream>>>(p);
@@ -650,7 +691,7 @@ struct GameVTable {
     int rot_records;  // rotated-sprite / span records per env (global)
     int blit_records; // blit list capacity per env (global)
     // [0] = the game's usual view, [1] = the whole-world view of center_agent = false (step[1] null: the game has none)
-    int setup_bytes[2];   // sizeof(FrameSetupT)
+    int setup_bytes[2];   // sizeof(FrameSharedT): the global record the setup kernel stores and the render kernel stages
     int cell_records[2];  // cells of the largest visible window (capacity for general cell blits)
     int frame_bytes[2];   // shared memory of one render CTA
     int render_ctas_per_sm[2];  // residency the render kernel is compiled for
@@ -664,7 +705,7 @@ struct GameVTable {
 template <class G, int VIEW>
 void fill_view(GameVTable &vt, int slot) {
     using F = FrameFor<G, VIEW>;
-    vt.setup_bytes[slot] = (int)sizeof(typename F::setup);
+    vt.setup_bytes[slot] = (int)sizeof(typename F::shared);
     vt.cell_records[slot] = F::type::kMaxCells1D * F::type::kMaxCells1D;
     vt.frame_bytes[slot] = (int)sizeof(typename F::type);
 #ifndef PG_HOSTSIM

@@ -103,7 +103,8 @@ constexpr uint32_t CI_FAST = 1u << 24;           // exactly one does
 //                 lookups, and the list of pre-scaled tiles to stage — everything that is O(entities
 //                 + cells) and heavy on fp64 or control flow. Lives in global memory; the render
 //                 CTA stages it into its shared memory with one bulk copy.
-//   FrameSetupT   + the setup kernel's own scratch (global, per env)
+//   FrameSetupT   + the setup kernel's own scratch. The whole record lives in the setup kernel's shared
+//                 memory, one per warp; only the FrameSharedT prefix is stored to global memory.
 //   FrameT        + the render kernel's scratch (shared memory): frame buffer, tile arena
 template <int MAX_CELLS_1D, int MAX_ENT_BLITS, int MAX_ROT_BLITS>
 struct alignas(16) FrameSharedT {
