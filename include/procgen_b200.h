@@ -299,7 +299,8 @@ LIBENV_API uint32_t pgb200_get_errors(libenv_env *handle, uint32_t *host_out);
 LIBENV_API int pgb200_debug_cycles(libenv_env *handle, uint32_t *host_out);
 
 /* Debug/inspection aid: copies env `env`'s header (512 B, layout csrc/pg_state.cuh EnvHdr) and up to
- * max_ents entity records (128 B each, csrc/pg_state.cuh Entity) to host memory; returns n_ents. */
+ * max_ents entity records (128 B each, csrc/pg_state.cuh Entity) to host memory; returns n_ents.
+ * Returns -1 and copies nothing when env is outside [0, num_envs). */
 LIBENV_API int pgb200_debug_read_env(libenv_env *handle, int env, void *hdr_out, void *ents_out, int max_ents);
 
 /* Peer mirror for the single gather of a sharded run (SURVEY §8e, BASELINE configs[4]): mirror0 / mirror1

@@ -39,6 +39,14 @@ static inline void pg_fatal(const char *fmt, ...) {
         if (_e != cudaSuccess)                                                                    \
             pg_fatal("CUDA error %s at %s:%d: %s\n", cudaGetErrorName(_e), __FILE__, __LINE__, cudaGetErrorString(_e)); \
     } while (0)
+using Stream = cudaStream_t;
+using Event = cudaEvent_t;
+#else
+// the host debug build has no streams or events: members of these types stay null there
+struct HostStream;
+struct HostEvent;
+using Stream = HostStream *;
+using Event = HostEvent *;
 #endif
 
 // ================================================================= kernels
@@ -444,15 +452,13 @@ void render_env_serial(const KParams &p, int env) {
 }
 
 struct LaunchCtx {
-#ifndef PG_HOSTSIM
-    cudaStream_t stream;
-    cudaStream_t logic_stream;  // null, or a higher-priority stream the logic kernel goes to (then `link` orders render behind it)
-    cudaEvent_t link;
+    Stream stream;
+    Stream logic_stream;      // null, or a higher-priority stream the logic kernel goes to (then `link` orders render behind it)
+    Event link;
     int max_logic_blocks;     // SM count x resident CTAs per SM
     int num_sms;              // SM count: sizes the machine-filling grids of a final-outputs step's phase B
     int render_smem_floor;    // dynamic shared memory requested per render CTA is at least this (co-residency knob)
-    cudaEvent_t *tev;         // optional: 4 events (before logic, after it, after setup, after render) for kernel timing
-#endif
+    Event *tev;               // optional: 4 events (before logic, after it, after setup, after render) for kernel timing
     // work counter of this launch slot (one per in-flight logic kernel); a two-phase step keeps its list's count and
     // phase B's ticket in the next two words
     unsigned int *ticket;

@@ -6,7 +6,13 @@
 //
 // Build modes: nvcc (product, sm_90a).  With -DPG_HOSTSIM the same file builds with g++ into the
 // CPU debug harness used ONLY by tests/ (every kernel becomes a plain loop); that build reports
-// pgb200_is_device_build() == 0 and the Python package refuses to load it.
+// pgb200_is_device_build() == 0 and the Python package refuses to load it. The two builds part ways
+// once for memory, copies and streams (the build seam below); past it they differ only where they do
+// different work: the device-only kernels, a step's stream fork / join and copies, device setup,
+// page-locking the caller's observations, and the entry points the host build refuses.
+//
+// A handle (VecEnv) owns every device array, pinned buffer, stream and event it creates: each is
+// registered with it when it is made, and ~VecEnv releases them all.
 #include <dlfcn.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -14,6 +20,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <random>
 #include <stdexcept>
 #include <string>
@@ -40,11 +47,6 @@
 #include "games/starpilot.cuh"
 #include "pg_state_io.h"
 
-#ifndef PG_HOSTSIM
-#include <cuda_fp16.h>
-#include <cuda_runtime.h>
-#endif
-
 namespace pg {
 const GameVTable *pg_vtable_bigfish();
 const GameVTable *pg_vtable_bossfight();
@@ -65,6 +67,78 @@ const GameVTable *pg_vtable_starpilot();
 }  // namespace pg
 
 using namespace pg;
+
+// ================================================================= build seam
+// What the runtime asks of CUDA, once per build. The host debug build keeps "device" memory on the heap,
+// copies with memcpy and finishes every launch before it returns: it has nothing to wait for and never captures.
+#ifndef PG_HOSTSIM
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+
+static constexpr int kDeviceBuild = 1;
+static inline void set_current_device(int device) { CUDA_CHECK(cudaSetDevice(device)); }
+// device memory, left as it is
+static inline void *dev_malloc(size_t bytes) {
+    void *ptr = nullptr;
+    CUDA_CHECK(cudaMalloc(&ptr, bytes));
+    return ptr;
+}
+static inline void dev_free(void *ptr) { cudaFree(ptr); }
+static inline void *pinned_alloc(size_t bytes) {
+    void *ptr = nullptr;
+    CUDA_CHECK(cudaHostAlloc(&ptr, bytes, cudaHostAllocDefault));
+    return ptr;
+}
+static inline void pinned_free(void *ptr) { cudaFreeHost(ptr); }
+static inline void host_unregister(void *ptr) { cudaHostUnregister(ptr); }
+static inline void stream_destroy(Stream s) { cudaStreamDestroy(s); }
+static inline void event_destroy(Event e) { cudaEventDestroy(e); }
+// on the legacy default stream, complete when they return
+static inline void dev_memset(void *dst, int value, size_t bytes) { CUDA_CHECK(cudaMemset(dst, value, bytes)); }
+static inline void copy_to_dev(void *dst, const void *src, size_t bytes) { CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); }
+static inline void copy_from_dev(void *dst, const void *src, size_t bytes) { CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); }
+// on stream s, behind the work issued there before
+static inline void copy_to_dev_async(void *dst, const void *src, size_t bytes, Stream s) {
+    CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s));
+}
+static inline void copy_from_dev_async(void *dst, const void *src, size_t bytes, Stream s) {
+    CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
+}
+static inline void memset_async(void *dst, int value, size_t bytes, Stream s) { CUDA_CHECK(cudaMemsetAsync(dst, value, bytes, s)); }
+static inline void stream_sync(Stream s) { CUDA_CHECK(cudaStreamSynchronize(s)); }
+static inline void device_sync() { CUDA_CHECK(cudaDeviceSynchronize()); }
+// Whether `s` is capturing a CUDA graph. Querying the legacy stream while another stream captures in a
+// non-relaxed mode reports cudaErrorStreamCaptureImplicit: work there would join that capture, so it counts.
+static inline bool stream_capturing(Stream s) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(s, &st);
+    if (e == cudaErrorStreamCaptureImplicit) {
+        cudaGetLastError();
+        return true;
+    }
+    CUDA_CHECK(e);
+    return st != cudaStreamCaptureStatusNone;
+}
+#else
+static constexpr int kDeviceBuild = 0;
+static inline void set_current_device(int) {}
+static inline void *dev_malloc(size_t bytes) { return calloc(bytes, 1); }
+static inline void dev_free(void *ptr) { free(ptr); }
+static inline void *pinned_alloc(size_t bytes) { return malloc(bytes); }
+static inline void pinned_free(void *ptr) { free(ptr); }
+static inline void host_unregister(void *) {}
+static inline void stream_destroy(Stream) {}
+static inline void event_destroy(Event) {}
+static inline void dev_memset(void *dst, int value, size_t bytes) { memset(dst, value, bytes); }
+static inline void copy_to_dev(void *dst, const void *src, size_t bytes) { memcpy(dst, src, bytes); }
+static inline void copy_from_dev(void *dst, const void *src, size_t bytes) { memcpy(dst, src, bytes); }
+static inline void copy_to_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
+static inline void copy_from_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
+static inline void memset_async(void *dst, int value, size_t bytes, Stream) { memset(dst, value, bytes); }
+static inline void stream_sync(Stream) {}
+static inline void device_sync() {}
+static inline bool stream_capturing(Stream) { return false; }
+#endif
 
 // ================================================================= option parsing (vecoptions.cpp)
 namespace {
@@ -145,43 +219,6 @@ const GameVTable *find_game(const std::string &name) {
     return nullptr;
 }
 
-// ================================================================= memory helpers
-template <class T>
-T *dev_alloc(size_t n) {
-    T *ptr = nullptr;
-    if (n == 0)
-        n = 1;
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMalloc((void **)&ptr, n * sizeof(T)));
-    CUDA_CHECK(cudaMemset(ptr, 0, n * sizeof(T)));
-#else
-    ptr = (T *)calloc(n, sizeof(T));
-#endif
-    return ptr;
-}
-void dev_free(void *ptr) {
-#ifndef PG_HOSTSIM
-    if (ptr)
-        cudaFree(ptr);
-#else
-    free(ptr);
-#endif
-}
-void copy_to_dev(void *dst, const void *src, size_t bytes) {
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
-#else
-    memcpy(dst, src, bytes);
-#endif
-}
-void copy_from_dev(void *dst, const void *src, size_t bytes) {
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
-#else
-    memcpy(dst, src, bytes);
-#endif
-}
-
 // vecgame.cpp:156-167: system-independent hash of the game name
 static int32_t fnv1a(const char *str) {
     uint32_t hash = 0x811c9dc5u;
@@ -192,16 +229,14 @@ static int32_t fnv1a(const char *str) {
     return (int32_t)hash;
 }
 
-// ================================================================= pre-scaled tile table
+// ================================================================= device-only kernels
 #ifndef PG_HOSTSIM
-// one CTA per (sprite slot, tw, th)
+// the pre-scaled tile table: one CTA per (sprite slot, tw, th)
 __global__ void tile_table_kernel(const SpriteDesc *sprites, const uint32_t *index, uint32_t *texels, const uint32_t *atlas) {
     const int slot = (int)blockIdx.x / TILE_VARIANTS, v = (int)blockIdx.x % TILE_VARIANTS;
     tile_table_fill(sprites, index, texels, atlas, slot, v / MAX_TILE_DIM + 1, v % MAX_TILE_DIM + 1, (int)threadIdx.x, (int)blockDim.x);
 }
-#endif
 
-#ifndef PG_HOSTSIM
 // (16-bit float)(v / 255.f) for v = 0..255: IEEE fp32 division, then round-to-nearest-even
 __global__ void consumer_lut_kernel(uint16_t *lut, int bf16) {
     const int v = (int)threadIdx.x;
@@ -217,19 +252,6 @@ __global__ void consumer_lut_kernel(uint16_t *lut, int bf16) {
 // The consumer ring position of the coming step, advanced on the device so that a step captured in a CUDA
 // graph moves it on at every replay (a kernel argument would be frozen at capture)
 __global__ void consumer_advance_kernel(int32_t *slot, int k) { *slot = (*slot + 1) % k; }
-
-// Whether `s` is capturing a CUDA graph. Querying the legacy stream while another stream captures in a
-// non-relaxed mode reports cudaErrorStreamCaptureImplicit: work there would join that capture, so it counts.
-static bool stream_capturing(cudaStream_t s) {
-    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
-    const cudaError_t e = cudaStreamIsCapturing(s, &st);
-    if (e == cudaErrorStreamCaptureImplicit) {
-        cudaGetLastError();
-        return true;
-    }
-    CUDA_CHECK(e);
-    return st != cudaStreamCaptureStatusNone;
-}
 #endif
 
 // ================================================================= VecEnv (VecGame, vecgame.h)
@@ -241,12 +263,8 @@ struct VecEnv {
     std::vector<libenv_tensortype> observation_types, action_types, info_types;
     int num_actions = -1;
 
-    KParams base{};                  // common launch parameters
+    KParams base{};                  // common launch parameters (a launch's own: game_params and its env range)
     std::vector<GameAssets *> d_assets;  // per joint game
-    uint32_t *d_atlas = nullptr;
-    uint32_t *d_tile_texels = nullptr, *d_tile_index = nullptr;
-    SpriteDesc *d_tile_sprites = nullptr;
-    uint32_t *d_lvl_seeds = nullptr;
     int32_t *d_action = nullptr;
     // The opt-in per-env arrays live in `base`, allocated by the first request for them (opt_in_array):
     // next_level_seed by pgb200_get_next_level_seeds; final_rgb and level_end by pgb200_get_final_outputs;
@@ -265,24 +283,28 @@ struct VecEnv {
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
 
-#ifndef PG_HOSTSIM
-    cudaStream_t stream = nullptr;
-    cudaStream_t own_stream = nullptr;
+    // everything the handle allocates or creates, registered as it is made (alloc, alloc_pinned, own, opt_in_array)
+    // and released by ~VecEnv
+    std::vector<void *> owned_dev, owned_pinned;
+    std::vector<Stream> owned_streams;
+    std::vector<Event> owned_events;
+
+    Stream stream = nullptr;  // where the handle's work goes: own_stream, or the caller's (pgb200_set_stream)
+    Stream own_stream = nullptr;
     static constexpr int kAuxStreams = PG_AUX_STREAMS;
-    cudaStream_t aux[kAuxStreams] = {};
+    Stream aux[kAuxStreams] = {};
     // PGB200_PRIORITY_SPLIT=1: logic kernels go to high-priority twins of the auxiliary streams so
     // their (small) blocks are dispatched ahead of the render CTAs queued by other chunks
     bool priority_split = false;
-    cudaStream_t aux_hi[kAuxStreams] = {};
-    cudaEvent_t ev_link[kAuxStreams] = {};
-    cudaEvent_t ev_fork = nullptr;
-    cudaEvent_t ev_join[kAuxStreams] = {};
-    // optional per-launch kernel timing (pgb200_kernel_timing_begin/end): a pool of event triples
-    std::vector<cudaEvent_t> tev_pool;
-    std::vector<int> tev_envs;   // env count of each timed launch pair
+    Stream aux_hi[kAuxStreams] = {};
+    Event ev_link[kAuxStreams] = {};
+    Event ev_fork = nullptr;
+    Event ev_join[kAuxStreams] = {};
+    // optional per-launch kernel timing (pgb200_kernel_timing_begin/end): a pool of event quadruples
+    std::vector<Event> tev_pool;
+    std::vector<int> tev_envs;   // env count of each timed launch
     size_t tev_used = 0;
     bool timing = false;
-#endif
     static constexpr int kChunks = PG_STEP_CHUNKS;
     int force_chunks = 0;            // measurement knobs (pgb200_set_launch_shape)
     bool serialize_launches = false;
@@ -290,7 +312,7 @@ struct VecEnv {
     // words per slot: the logic kernel's ticket; with final outputs also the pending-reset count and phase B's ticket
     static constexpr int kTicketWords = 4;
     unsigned int *d_tickets = nullptr;
-    int max_logic_blocks = 1 << 30;
+    int max_logic_blocks = 1;        // logic blocks the device holds at once (device setup); the host build runs one env at a time
     int num_sms = 1;
     int render_smem_floor = 0;
     // host-buffer (libenv) mode
@@ -319,9 +341,43 @@ struct VecEnv {
     uint8_t *st_prev_complete = nullptr;
     int32_t *st_seed = nullptr;
 
+    VecEnv() = default;
+    VecEnv(const VecEnv &) = delete;
+    VecEnv &operator=(const VecEnv &) = delete;
+    ~VecEnv() {
+        for (void *ptr : owned_dev) dev_free(ptr);
+        for (void *ptr : owned_pinned) pinned_free(ptr);
+        for (Event e : owned_events) event_destroy(e);
+        for (Stream s : owned_streams) stream_destroy(s);
+    }
+
+    // A device array of n elements (at least one), zero-filled on the legacy stream, that the handle owns
+    template <class T>
+    T *alloc(size_t n) {
+        const size_t bytes = (n ? n : 1) * sizeof(T);
+        void *ptr = dev_malloc(bytes);
+        owned_dev.push_back(ptr);
+        dev_memset(ptr, 0, bytes);
+        return (T *)ptr;
+    }
+    // A pinned host buffer of n elements (at least one) that the handle owns
+    template <class T>
+    T *alloc_pinned(size_t n) {
+        void *ptr = pinned_alloc((n ? n : 1) * sizeof(T));
+        owned_pinned.push_back(ptr);
+        return (T *)ptr;
+    }
+    Stream own(Stream s) {
+        owned_streams.push_back(s);
+        return s;
+    }
+    Event own(Event e) {
+        owned_events.push_back(e);
+        return e;
+    }
+
     LaunchCtx lctx() {
         LaunchCtx lc;
-#ifndef PG_HOSTSIM
         lc.stream = stream;
         lc.logic_stream = nullptr;
         lc.link = nullptr;
@@ -329,10 +385,21 @@ struct VecEnv {
         lc.num_sms = num_sms;
         lc.render_smem_floor = render_smem_floor;
         lc.tev = nullptr;
-#endif
         lc.ticket = d_tickets;
         lc.launch_counter = &launches;
         return lc;
+    }
+
+    // `base` as the launches of joint game g see it: the game's assets, id and fixed asset seed, and its slots of the
+    // level bank if there is one. The caller sets the launch's env range.
+    KParams game_params(int g) const {
+        KParams p = base;
+        p.assets = d_assets[g];
+        p.game_id = games[g]->id;
+        p.fixed_asset_seed = fnv1a(games[g]->name);
+        if (base.bank.slots)
+            p.bank = banks[g];
+        return p;
     }
 
     // One step = for every (game, env chunk): logic kernel then render kernel. Chunks go round-robin
@@ -345,6 +412,9 @@ struct VecEnv {
         int chunks = force_chunks > 0 ? force_chunks : kChunks;
         if (force_chunks <= 0 && per_game < 4096 * chunks)
             chunks = 1;
+        // more than one (logic, render) pair in the step — env chunks of one game, or the games of a
+        // joint list — are spread over the auxiliary streams so they overlap on the SMs
+        const int nstreams = (chunks * G > 1 && !serialize_launches) ? kAuxStreams : 0;
 #ifndef PG_HOSTSIM
         // the consumer ring moves on once per step, behind the previous step and ahead of every render
         // kernel of this one (they all start after the fork below)
@@ -353,9 +423,6 @@ struct VecEnv {
             CUDA_CHECK(cudaGetLastError());
             launches++;
         }
-        // more than one (logic, render) pair in the step — env chunks of one game, or the games of a
-        // joint list — are spread over the auxiliary streams so they overlap on the SMs
-        const int nstreams = (chunks * G > 1 && !serialize_launches) ? kAuxStreams : 0;
         if (nstreams) {
             CUDA_CHECK(cudaEventRecord(ev_fork, stream));
             for (int s = 0; s < nstreams; s++) {
@@ -376,20 +443,14 @@ struct VecEnv {
             for (int cidx = 0; cidx < chunks; cidx++, k++) {
                 const int lo = (int)((int64_t)per_game * cidx / chunks);
                 const int hi = (int)((int64_t)per_game * (cidx + 1) / chunks);
-                KParams p = base;
-                p.assets = d_assets[g];
-                p.game_id = games[g]->id;
-                p.fixed_asset_seed = fnv1a(games[g]->name);
+                KParams p = game_params(g);
                 p.env_first = g + lo * G;
                 p.env_step = G;
                 p.env_count = hi - lo;
                 if (base.reset_list)
                     p.reset_list = base.reset_list + g * per_game + lo;  // the launch's own segment
-                if (base.bank.slots)
-                    p.bank = banks[g];
                 LaunchCtx lc = lctx();
                 lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
-#ifndef PG_HOSTSIM
                 if (nstreams) {
                     lc.stream = aux[k % nstreams];
                     if (priority_split) {
@@ -402,7 +463,6 @@ struct VecEnv {
                     tev_used += 4;
                     tev_envs.push_back(p.env_count);
                 }
-#endif
                 if (init)
                     games[g]->init[view[g]](p, lc);
                 else
@@ -451,25 +511,27 @@ struct VecEnv {
         initial_reset_done = true;
     }
 
-    void sync() {
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaStreamSynchronize(stream));
-#endif
-    }
+    void sync() { stream_sync(stream); }
 
     // True while the handle's stream captures a CUDA graph. The entry points that wait for the device or
     // allocate then refuse (-1, or a fatal message where the call returns nothing): either would
     // invalidate the caller's capture.
-    bool capturing() {
-#ifndef PG_HOSTSIM
-        return stream_capturing(stream);
-#else
-        return false;
-#endif
-    }
+    bool capturing() { return stream_capturing(stream); }
     void refuse_in_capture(const char *what) {
         if (capturing())
             pg_fatal("%s cannot run while the handle's stream is capturing a CUDA graph\n", what);
+    }
+
+    // The start of an entry point that waits for the device and returns an error value (-1, or UINT32_MAX): false
+    // while the handle's stream captures. Otherwise true once the stream has finished its work, the initial reset
+    // included when `initial_reset` asks for it.
+    bool try_sync(bool initial_reset = false) {
+        if (capturing())
+            return false;
+        if (initial_reset)
+            ensure_initial_reset();
+        sync();
+        return true;
     }
 
     // The start of an entry point that hands out an opt-in array: false (the entry point returns -1) while the
@@ -482,28 +544,21 @@ struct VecEnv {
         return true;
     }
 
-    // An opt-in per-env array of `per_env` elements per env, allocated at the first request (ptr null) with every
-    // byte set to `fill` on the handle's stream, which completes before the caller uses it from any stream
+    // An opt-in per-env array of `per_env` elements per env that the handle owns, allocated at the first request
+    // (ptr null) with every byte set to `fill` on the handle's stream, which completes before the caller uses it
+    // from any stream
     template <class T>
     void opt_in_array(T *&ptr, size_t per_env, int fill) {
         if (ptr)
             return;
         const size_t bytes = (num_envs ? (size_t)num_envs : 1) * per_env * sizeof(T);
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaMalloc((void **)&ptr, bytes));
-        CUDA_CHECK(cudaMemsetAsync(ptr, fill, bytes, stream));
-#else
-        ptr = (T *)malloc(bytes);
-        memset(ptr, fill, bytes);
-#endif
+        ptr = (T *)dev_malloc(bytes);
+        owned_dev.push_back(ptr);
+        memset_async(ptr, fill, bytes, stream);
         sync();
     }
 
-    void set_device() {
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaSetDevice(device));
-#endif
-    }
+    void set_device() { set_current_device(device); }
 };
 
 std::string default_pack_path() {
@@ -571,13 +626,7 @@ extern "C" {
 
 int libenv_version(void) { return LIBENV_VERSION; }
 
-int pgb200_is_device_build(void) {
-#ifndef PG_HOSTSIM
-    return 1;
-#else
-    return 0;
-#endif
-}
+int pgb200_is_device_build(void) { return kDeviceBuild; }
 
 libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
     OptParser opts(options);
@@ -670,8 +719,17 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
         CUDA_CHECK(cudaGetDevice(&cuda_device));
     v->device = cuda_device;
     v->set_device();
-    CUDA_CHECK(cudaStreamCreateWithFlags(&v->own_stream, cudaStreamNonBlocking));
-    v->stream = v->own_stream;
+    auto new_stream = [v] {
+        cudaStream_t s = nullptr;
+        CUDA_CHECK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+        return v->own(s);
+    };
+    auto new_event = [v] {
+        cudaEvent_t e = nullptr;
+        CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        return v->own(e);
+    };
+    v->stream = v->own_stream = new_stream();
     {
         const char *e = getenv("PGB200_PRIORITY_SPLIT");
         v->priority_split = e && atoi(e) != 0;
@@ -679,14 +737,16 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
     int prio_lo = 0, prio_hi = 0;
     CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));  // numerically lower = higher priority
     for (int s = 0; s < VecEnv::kAuxStreams; s++) {
-        CUDA_CHECK(cudaStreamCreateWithFlags(&v->aux[s], cudaStreamNonBlocking));
-        CUDA_CHECK(cudaEventCreateWithFlags(&v->ev_join[s], cudaEventDisableTiming));
+        v->aux[s] = new_stream();
+        v->ev_join[s] = new_event();
         if (v->priority_split) {
-            CUDA_CHECK(cudaStreamCreateWithPriority(&v->aux_hi[s], cudaStreamNonBlocking, prio_hi));
-            CUDA_CHECK(cudaEventCreateWithFlags(&v->ev_link[s], cudaEventDisableTiming));
+            cudaStream_t hi = nullptr;
+            CUDA_CHECK(cudaStreamCreateWithPriority(&hi, cudaStreamNonBlocking, prio_hi));
+            v->aux_hi[s] = v->own(hi);
+            v->ev_link[s] = new_event();
         }
     }
-    CUDA_CHECK(cudaEventCreateWithFlags(&v->ev_fork, cudaEventDisableTiming));
+    v->ev_fork = new_event();
     {
         cudaDeviceProp prop;
         CUDA_CHECK(cudaGetDeviceProperties(&prop, v->device));
@@ -705,7 +765,7 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
             v->render_smem_floor = (227 * 1024) / render_ctas - 1024 - 16;
             v->render_smem_floor &= ~15;
         }
-        v->d_consumer_slot = dev_alloc<int32_t>(1);
+        v->d_consumer_slot = v->alloc<int32_t>(1);
         v->base.consumer_slot_dev = v->d_consumer_slot;
     }
     // sub_step <-> push_obj recurse to depth 5 on the logic thread
@@ -715,10 +775,8 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
         if (cur < 4096)  // only ever raise it: the host application may have asked for more
             CUDA_CHECK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
     }
-#else
-    v->device = -1;
 #endif
-    v->d_tickets = dev_alloc<unsigned int>(VecEnv::kMaxTickets * VecEnv::kTicketWords);
+    v->d_tickets = v->alloc<unsigned int>(VecEnv::kMaxTickets * VecEnv::kTicketWords);
 
     // ---- assets
     std::string pack_path = resource_root;
@@ -735,10 +793,11 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
         host::AtlasBuilder atlas(pack);
         std::vector<GameAssets> tables(G);
         for (int g = 0; g < G; g++) atlas.build_game(v->games[g]->id, tables[g]);
-        v->d_atlas = dev_alloc<uint32_t>(atlas.texels.size());
-        copy_to_dev(v->d_atlas, atlas.texels.data(), atlas.texels.size() * sizeof(uint32_t));
+        uint32_t *atlas_texels = v->alloc<uint32_t>(atlas.texels.size());
+        copy_to_dev(atlas_texels, atlas.texels.data(), atlas.texels.size() * sizeof(uint32_t));
+        v->base.atlas = atlas_texels;
         for (int g = 0; g < G; g++) {
-            GameAssets *d = dev_alloc<GameAssets>(1);
+            GameAssets *d = v->alloc<GameAssets>(1);
             copy_to_dev(d, &tables[g], sizeof(GameAssets));
             v->d_assets.push_back(d);
         }
@@ -757,22 +816,22 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
                     }
             if (top >= (size_t)1 << 32)
                 throw std::runtime_error("tile table too large");
-            v->d_tile_index = dev_alloc<uint32_t>(index.size());
-            copy_to_dev(v->d_tile_index, index.data(), index.size() * sizeof(uint32_t));
-            v->d_tile_sprites = dev_alloc<SpriteDesc>((size_t)S);
-            copy_to_dev(v->d_tile_sprites, atlas.tile_sprites.data(), (size_t)S * sizeof(SpriteDesc));
-            v->d_tile_texels = dev_alloc<uint32_t>(top);
+            uint32_t *tile_index = v->alloc<uint32_t>(index.size());
+            copy_to_dev(tile_index, index.data(), index.size() * sizeof(uint32_t));
+            SpriteDesc *tile_sprites = v->alloc<SpriteDesc>((size_t)S);
+            copy_to_dev(tile_sprites, atlas.tile_sprites.data(), (size_t)S * sizeof(SpriteDesc));
+            uint32_t *tile_texels = v->alloc<uint32_t>(top);
 #ifndef PG_HOSTSIM
-            tile_table_kernel<<<S * TILE_VARIANTS, 64>>>(v->d_tile_sprites, v->d_tile_index, v->d_tile_texels, v->d_atlas);
+            tile_table_kernel<<<S * TILE_VARIANTS, 64>>>(tile_sprites, tile_index, tile_texels, atlas_texels);
             CUDA_CHECK(cudaGetLastError());
 #else
             for (int sl = 0; sl < S; sl++)
                 for (int vv = 0; vv < TILE_VARIANTS; vv++)
-                    tile_table_fill(v->d_tile_sprites, v->d_tile_index, v->d_tile_texels, v->d_atlas, sl, vv / MAX_TILE_DIM + 1, vv % MAX_TILE_DIM + 1, 0, 1);
+                    tile_table_fill(tile_sprites, tile_index, tile_texels, atlas_texels, sl, vv / MAX_TILE_DIM + 1, vv % MAX_TILE_DIM + 1, 0, 1);
 #endif
-            v->base.tiles.texels = v->d_tile_texels;
-            v->base.tiles.index = v->d_tile_index;
-            v->base.tiles.sprites = v->d_tile_sprites;
+            v->base.tiles.texels = tile_texels;
+            v->base.tiles.index = tile_index;
+            v->base.tiles.sprites = tile_sprites;
             v->base.tiles.n_slots = S;
         }
     } catch (const std::exception &e) {
@@ -798,31 +857,29 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
     p.ent_stride = ent_cap + 1;
     p.grid_stride = grid_cap;
     p.scratch_stride = scratch_words;
-    p.hdr = dev_alloc<EnvHdr>(N);
-    p.ents = dev_alloc<Entity>(N * p.ent_stride);
-    p.grid = dev_alloc<int16_t>(N * p.grid_stride);
-    p.rng = dev_alloc<MT19937>(N);
-    p.lvl_rng = dev_alloc<MT19937>(N);
-    p.scratch = dev_alloc<int32_t>(N * (size_t)scratch_words);
+    p.hdr = v->alloc<EnvHdr>(N);
+    p.ents = v->alloc<Entity>(N * p.ent_stride);
+    p.grid = v->alloc<int16_t>(N * p.grid_stride);
+    p.rng = v->alloc<MT19937>(N);
+    p.lvl_rng = v->alloc<MT19937>(N);
+    p.scratch = v->alloc<int32_t>(N * (size_t)scratch_words);
     p.rot_stride = rot_records;
-    p.rot_scratch = rot_records > 0 ? dev_alloc<RotBlit>(N * (size_t)rot_records) : nullptr;
+    p.rot_scratch = rot_records > 0 ? v->alloc<RotBlit>(N * (size_t)rot_records) : nullptr;
     p.blit_stride = blit_records;
-    p.blit_list = dev_alloc<Blit>(N * (size_t)blit_records);
+    p.blit_list = v->alloc<Blit>(N * (size_t)blit_records);
     p.cell_spill_stride = cell_records;
-    p.cell_spill = dev_alloc<Blit>(N * (size_t)cell_records);
+    p.cell_spill = v->alloc<Blit>(N * (size_t)cell_records);
     p.frame_setup_stride = (setup_bytes + 15) & ~15;
-    p.frame_setup = dev_alloc<unsigned char>(N * (size_t)p.frame_setup_stride);
-    p.atlas = v->d_atlas;
-    v->d_action = dev_alloc<int32_t>(N);
+    p.frame_setup = v->alloc<unsigned char>(N * (size_t)p.frame_setup_stride);
+    v->d_action = v->alloc<int32_t>(N);
     p.action = v->d_action;
-    p.rgb = dev_alloc<uint8_t>(N * RES_W * RES_H * 3);
-    p.rew = dev_alloc<float>(N);
-    p.first = dev_alloc<uint8_t>(N);
-    p.info_prev_level_seed = dev_alloc<int32_t>(N);
-    p.info_prev_level_complete = dev_alloc<uint8_t>(N);
-    p.info_level_seed = dev_alloc<int32_t>(N);
-    p.dbg_cycles = getenv("PGB200_DEBUG_TIMING") ? dev_alloc<uint32_t>(N) : nullptr;
-
+    p.rgb = v->alloc<uint8_t>(N * RES_W * RES_H * 3);
+    p.rew = v->alloc<float>(N);
+    p.first = v->alloc<uint8_t>(N);
+    p.info_prev_level_seed = v->alloc<int32_t>(N);
+    p.info_prev_level_complete = v->alloc<uint8_t>(N);
+    p.info_level_seed = v->alloc<int32_t>(N);
+    p.dbg_cycles = getenv("PGB200_DEBUG_TIMING") ? v->alloc<uint32_t>(N) : nullptr;
 
     // ---- per-env seed chain (vecgame.cpp:301-314), replayed for the global env indices
     {
@@ -831,9 +888,9 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
         for (int i = 0; i < env_index_offset; i++) (void)game_level_seed_gen();
         std::vector<uint32_t> seeds(N);
         for (size_t i = 0; i < N; i++) seeds[i] = (uint32_t)game_level_seed_gen();
-        v->d_lvl_seeds = dev_alloc<uint32_t>(N);
-        copy_to_dev(v->d_lvl_seeds, seeds.data(), N * sizeof(uint32_t));
-        p.lvl_seeds = v->d_lvl_seeds;
+        uint32_t *lvl_seeds = v->alloc<uint32_t>(N);
+        copy_to_dev(lvl_seeds, seeds.data(), N * sizeof(uint32_t));
+        p.lvl_seeds = lvl_seeds;
     }
 
     // vecgame.cpp:284-293
@@ -860,11 +917,9 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
     p.options.distribution_mode = dist_mode;
     p.snap = snap ? 1 : 0;
     p.env_global_offset = env_index_offset;
-#ifndef PG_HOSTSIM
     // every upload and memset above ran on the legacy default stream; the step kernels run on
     // non-blocking streams that do not order against it
-    CUDA_CHECK(cudaDeviceSynchronize());
-#endif
+    device_sync();
     return (libenv_env *)v;
 }
 
@@ -884,47 +939,19 @@ int libenv_get_tensortypes(libenv_env *handle, enum libenv_space_name name, stru
     return (int)types->size();
 }
 
-static void *host_alloc(size_t bytes) {
-#ifndef PG_HOSTSIM
-    void *ptr = nullptr;
-    CUDA_CHECK(cudaHostAlloc(&ptr, bytes ? bytes : 1, cudaHostAllocDefault));
-    return ptr;
-#else
-    return malloc(bytes ? bytes : 1);
-#endif
-}
-static void host_free(void *ptr) {
-#ifndef PG_HOSTSIM
-    if (ptr)
-        cudaFreeHost(ptr);
-#else
-    free(ptr);
-#endif
-}
-
-// device -> host on the handle's stream, ordered behind its kernels (host build: memcpy)
-static void copy_from_dev_async(VecEnv *v, void *dst, const void *src, size_t bytes) {
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, v->stream));
-#else
-    (void)v;
-    memcpy(dst, src, bytes);
-#endif
-}
-
 static void fetch_to_host(VecEnv *v) {
     const size_t N = (size_t)v->num_envs;
     const KParams &p = v->base;
     const size_t frame = RES_W * RES_H * 3;
     uint8_t *rgb_dst = v->ob_direct ? (uint8_t *)v->h_ob[0] : v->st_rgb;
     if (!v->rgb_copy_enqueued)
-        copy_from_dev_async(v, rgb_dst, p.rgb, N * frame);
+        copy_from_dev_async(rgb_dst, p.rgb, N * frame, v->stream);
     v->rgb_copy_enqueued = false;
-    copy_from_dev_async(v, v->st_rew, p.rew, N * sizeof(float));
-    copy_from_dev_async(v, v->st_first, p.first, N);
-    copy_from_dev_async(v, v->st_prev_seed, p.info_prev_level_seed, N * 4);
-    copy_from_dev_async(v, v->st_prev_complete, p.info_prev_level_complete, N);
-    copy_from_dev_async(v, v->st_seed, p.info_level_seed, N * 4);
+    copy_from_dev_async(v->st_rew, p.rew, N * sizeof(float), v->stream);
+    copy_from_dev_async(v->st_first, p.first, N, v->stream);
+    copy_from_dev_async(v->st_prev_seed, p.info_prev_level_seed, N * 4, v->stream);
+    copy_from_dev_async(v->st_prev_complete, p.info_prev_level_complete, N, v->stream);
+    copy_from_dev_async(v->st_seed, p.info_level_seed, N * 4, v->stream);
     v->sync();
     if (!v->ob_direct)
         for (size_t e = 0; e < N; e++) memcpy(v->h_ob[e], v->st_rgb + e * frame, frame);
@@ -977,13 +1004,13 @@ void libenv_set_buffers(libenv_env *handle, struct libenv_buffers *bufs) {
         v->ob_direct = contiguous;
 #endif
     }
-    v->st_rgb = v->ob_direct ? nullptr : (uint8_t *)host_alloc(N * RES_W * RES_H * 3);
-    v->st_action = (int32_t *)host_alloc(N * 4);
-    v->st_rew = (float *)host_alloc(N * 4);
-    v->st_first = (uint8_t *)host_alloc(N);
-    v->st_prev_seed = (int32_t *)host_alloc(N * 4);
-    v->st_prev_complete = (uint8_t *)host_alloc(N);
-    v->st_seed = (int32_t *)host_alloc(N * 4);
+    v->st_rgb = v->ob_direct ? nullptr : v->alloc_pinned<uint8_t>(N * RES_W * RES_H * 3);
+    v->st_action = v->alloc_pinned<int32_t>(N);
+    v->st_rew = v->alloc_pinned<float>(N);
+    v->st_first = v->alloc_pinned<uint8_t>(N);
+    v->st_prev_seed = v->alloc_pinned<int32_t>(N);
+    v->st_prev_complete = v->alloc_pinned<uint8_t>(N);
+    v->st_seed = v->alloc_pinned<int32_t>(N);
     v->ensure_initial_reset();  // vecgame.cpp:349-353
 }
 
@@ -1003,11 +1030,7 @@ void libenv_act(libenv_env *handle) {
     const size_t N = (size_t)v->num_envs;
     v->sync();  // staging buffer reuse (wait_for_stepping_threads, vecgame.cpp:379)
     for (size_t e = 0; e < N; e++) v->st_action[e] = *(int32_t *)v->h_ac[e];
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpyAsync(v->d_action, v->st_action, N * 4, cudaMemcpyHostToDevice, v->stream));
-#else
-    memcpy(v->d_action, v->st_action, N * 4);
-#endif
+    copy_to_dev_async(v->d_action, v->st_action, N * 4, v->stream);
     v->launch(false);
 }
 
@@ -1018,77 +1041,9 @@ void libenv_close(libenv_env *handle) {
     v->set_device();
     v->refuse_in_capture("libenv_close");
     v->sync();
-    KParams &p = v->base;
-    dev_free(p.hdr);
-    dev_free(p.ents);
-    dev_free(p.grid);
-    dev_free(p.rng);
-    dev_free(p.lvl_rng);
-    dev_free(p.scratch);
-    if (p.rot_scratch)
-        dev_free(p.rot_scratch);
-    dev_free(p.blit_list);
-    dev_free(p.frame_setup);
-    dev_free(p.cell_spill);
-    dev_free(v->d_atlas);
-    dev_free(v->d_tile_texels);
-    dev_free(v->d_tile_index);
-    dev_free(v->d_tile_sprites);
-    dev_free(v->d_action);
-    dev_free(p.next_level_seed);
-    dev_free(p.final_rgb);
-    dev_free(p.level_end);
-    dev_free(p.reset_list);
-    dev_free(v->d_pause);
-    dev_free(p.paused);
-    dev_free(p.bank.slots);
-    dev_free(p.bank_level_end);
-    dev_free(v->d_bank_seeds);
-    dev_free(v->d_bank_count);
-    dev_free(p.rgb);
-    dev_free(p.rew);
-    dev_free(p.first);
-    dev_free(p.info_prev_level_seed);
-    dev_free(p.info_prev_level_complete);
-    dev_free(p.info_level_seed);
-    dev_free(v->d_lvl_seeds);
-    dev_free(v->d_consumer_lut);
-    dev_free(v->d_consumer_slot);
-    if (p.dbg_cycles)
-        dev_free(p.dbg_cycles);
-#ifndef PG_HOSTSIM
-    for (cudaEvent_t e : v->tev_pool) cudaEventDestroy(e);
-#endif
-    dev_free(v->d_tickets);
-    for (auto a : v->d_assets) dev_free(a);
-    host_free(v->st_rgb);
-#ifndef PG_HOSTSIM
     if (v->ob_registered)
-        cudaHostUnregister(v->h_ob[0]);
-#endif
-    host_free(v->st_action);
-    host_free(v->st_rew);
-    host_free(v->st_first);
-    host_free(v->st_prev_seed);
-    host_free(v->st_prev_complete);
-    host_free(v->st_seed);
-#ifndef PG_HOSTSIM
-    for (int s = 0; s < VecEnv::kAuxStreams; s++) {
-        if (v->aux[s])
-            cudaStreamDestroy(v->aux[s]);
-        if (v->aux_hi[s])
-            cudaStreamDestroy(v->aux_hi[s]);
-        if (v->ev_link[s])
-            cudaEventDestroy(v->ev_link[s]);
-        if (v->ev_join[s])
-            cudaEventDestroy(v->ev_join[s]);
-    }
-    if (v->ev_fork)
-        cudaEventDestroy(v->ev_fork);
-    if (v->own_stream)
-        cudaStreamDestroy(v->own_stream);
-#endif
-    delete v;
+        host_unregister(v->h_ob[0]);
+    delete v;  // releases everything the handle allocated or created
 }
 
 int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *out) {
@@ -1107,11 +1062,7 @@ int pgb200_get_device_buffers(libenv_env *handle, struct pgb200_device_buffers *
     out->action = v->d_action;
     out->num_envs = v->num_envs;
     out->device = v->device;
-#ifndef PG_HOSTSIM
     out->stream = (void *)v->stream;
-#else
-    out->stream = nullptr;
-#endif
     return 0;
 }
 
@@ -1170,8 +1121,8 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
     const int G = (int)v->games.size();
     if (!base.bank.slots) {
         v->bank_capacity = std::max(count, capacity);
-        v->d_bank_seeds = dev_alloc<int32_t>((size_t)v->bank_capacity);
-        v->d_bank_count = dev_alloc<int32_t>(1);
+        v->d_bank_seeds = v->alloc<int32_t>((size_t)v->bank_capacity);
+        v->d_bank_count = v->alloc<int32_t>(1);
         // a banked step lists its resets as a step with final outputs does (launch_step)
         v->opt_in_array(base.bank_level_end, 1, 0);
         v->opt_in_array(base.reset_list, 1, 0);
@@ -1191,47 +1142,29 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
             total += (size_t)v->bank_capacity * b.slot_bytes;
             v->banks.push_back(b);
         }
-        unsigned char *slots = dev_alloc<unsigned char>(total);
+        unsigned char *slots = v->alloc<unsigned char>(total);
         for (LevelBank &b : v->banks) b.slots = slots + reinterpret_cast<size_t>(b.slots);
         v->bank_bytes = (int64_t)total + (int64_t)v->bank_capacity * (int64_t)sizeof(int32_t) + (int64_t)sizeof(int32_t);
         // set last: a non-null slots pointer is what selects the bank's kernels
         base.bank = v->banks[0];
         base.bank.slots = slots;
-#ifndef PG_HOSTSIM
-        CUDA_CHECK(cudaDeviceSynchronize());  // dev_alloc's memsets ran on the legacy stream
-#endif
+        device_sync();  // alloc's memsets ran on the legacy stream
     }
-    // staging of the build's warps (a level generated at the env's own capacities), bounded by a fixed budget
+    // staging of the build's warps (a level generated at the env's own capacities), bounded by a fixed budget, and
+    // released when the build has finished with it
     const size_t stage_bytes = bank_stage_bytes(base);
     int warps = (int)std::min<size_t>((size_t)std::max(n, 1), std::max<size_t>(((size_t)256 << 20) / stage_bytes, 1));
-#ifndef PG_HOSTSIM
     warps = std::min(warps, v->max_logic_blocks * kLogicEnvsPerBlock);
-    unsigned char *stage = nullptr;
-    CUDA_CHECK(cudaMalloc((void **)&stage, (size_t)warps * stage_bytes));
+    std::unique_ptr<unsigned char, void (*)(void *)> stage((unsigned char *)dev_malloc((size_t)warps * stage_bytes), dev_free);
     // ordered behind every step issued so far, and every later step behind the rebuild
-    CUDA_CHECK(cudaMemcpyAsync(v->d_bank_seeds, sorted.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, v->stream));
-#else
-    unsigned char *stage = (unsigned char *)calloc(stage_bytes, 1);
-    memcpy(v->d_bank_seeds, sorted.data(), (size_t)n * sizeof(int32_t));
-#endif
+    copy_to_dev_async(v->d_bank_seeds, sorted.data(), (size_t)n * sizeof(int32_t), v->stream);
     for (int g = 0; g < G; g++) {
-        KParams p = base;
-        p.assets = v->d_assets[g];
-        p.game_id = v->games[g]->id;
-        p.fixed_asset_seed = fnv1a(v->games[g]->name);
-        p.bank = v->banks[g];
         LaunchCtx lc = v->lctx();
-        v->games[g]->bank_build(p, lc, stage, warps, n);
+        v->games[g]->bank_build(v->game_params(g), lc, stage.get(), warps, n);
     }
-#ifndef PG_HOSTSIM
     const int32_t n_dev = n;
-    CUDA_CHECK(cudaMemcpyAsync(v->d_bank_count, &n_dev, sizeof(int32_t), cudaMemcpyHostToDevice, v->stream));
+    copy_to_dev_async(v->d_bank_count, &n_dev, sizeof(int32_t), v->stream);
     v->sync();  // the host sources above, then the staging
-    CUDA_CHECK(cudaFree(stage));
-#else
-    *v->d_bank_count = n;
-    free(stage);
-#endif
     v->bank_levels = n;
     return 0;
 }
@@ -1248,26 +1181,20 @@ int pgb200_level_bank_info(libenv_env *handle, int *levels, int64_t *bytes) {
 void pgb200_set_stream(libenv_env *handle, void *stream) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-#ifndef PG_HOSTSIM
-    cudaStream_t next = (stream == PGB200_PRIVATE_STREAM) ? v->own_stream : (cudaStream_t)stream;
+    const Stream next = (stream == PGB200_PRIVATE_STREAM) ? v->own_stream : (Stream)stream;
     // a stream that is capturing cannot be waited on, neither the new one nor the old one: moving into a
     // capture, the caller has ordered the handle's earlier work before the capture began
     if (!stream_capturing(next) && !v->capturing())
         v->sync();
     v->stream = next;
-#else
-    v->sync();
-    (void)stream;
-#endif
 }
 
 int pgb200_set_rgb_mirror(libenv_env *handle, void *mirror0, void *mirror1) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing())
+    if (!v->try_sync())
         return -1;
-    v->sync();
     v->mirror[0] = (uint8_t *)mirror0;
     v->mirror[1] = (uint8_t *)(mirror1 ? mirror1 : mirror0);
     v->mirror_parity = 0;
@@ -1282,10 +1209,8 @@ int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int 
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing())
+    if (!v->try_sync(true))
         return -1;
-    v->ensure_initial_reset();
-    v->sync();
     if (buffer == nullptr || dtype == 0) {
         v->base.consumer = nullptr;
         return 0;
@@ -1293,7 +1218,7 @@ int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int 
     if ((dtype != 1 && dtype != 2) || k_frames < 1 || k_frames > 16)
         return -1;
     if (!v->d_consumer_lut)
-        v->d_consumer_lut = dev_alloc<uint16_t>(256);
+        v->d_consumer_lut = v->alloc<uint16_t>(256);
     consumer_lut_kernel<<<1, 256, 0, v->stream>>>(v->d_consumer_lut, dtype == 2);
     CUDA_CHECK(cudaGetLastError());
     v->base.consumer = buffer;
@@ -1301,12 +1226,10 @@ int pgb200_set_consumer_output(libenv_env *handle, void *buffer, int dtype, int 
     v->base.consumer_k = k_frames;
     v->consumer_slot = 0;
     v->consumer_steps = 0;
-    CUDA_CHECK(cudaMemsetAsync(v->d_consumer_slot, 0, sizeof(int32_t), v->stream));
+    memset_async(v->d_consumer_slot, 0, sizeof(int32_t), v->stream);
     // the current frame of every env becomes the newest frame of an otherwise empty stack
     for (size_t g = 0; g < v->games.size(); g++) {
-        KParams p = v->base;
-        p.assets = v->d_assets[g];
-        p.game_id = v->games[g]->id;
+        KParams p = v->game_params((int)g);
         p.env_first = (int)g;
         p.env_step = (int)v->games.size();
         p.env_count = v->num_envs / (int)v->games.size();
@@ -1381,9 +1304,8 @@ void pgb200_sync(libenv_env *handle) {
 uint32_t pgb200_get_errors(libenv_env *handle, uint32_t *host_out) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing())
+    if (!v->try_sync())
         return UINT32_MAX;
-    v->sync();
     const size_t N = (size_t)v->num_envs;
     std::vector<EnvHdr> hdr(N);
     copy_from_dev(hdr.data(), v->base.hdr, N * sizeof(EnvHdr));
@@ -1401,21 +1323,19 @@ int pgb200_debug_cycles(libenv_env *handle, uint32_t *host_out) {
     if (!v->base.dbg_cycles)
         return -1;
     v->set_device();
-    if (v->capturing())
+    if (!v->try_sync())
         return -1;
-    v->sync();
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaMemcpy(host_out, v->base.dbg_cycles, (size_t)v->num_envs * 4, cudaMemcpyDeviceToHost));
-#endif
+    copy_from_dev(host_out, v->base.dbg_cycles, (size_t)v->num_envs * 4);
     return 0;
 }
 
 int pgb200_debug_read_env(libenv_env *handle, int env, void *hdr_out, void *ents_out, int max_ents) {
     VecEnv *v = (VecEnv *)handle;
-    v->set_device();
-    if (v->capturing())
+    if (env < 0 || env >= v->num_envs)
         return -1;
-    v->sync();
+    v->set_device();
+    if (!v->try_sync())
+        return -1;
     EnvHdr hdr;
     const KParams &p = v->base;
     copy_from_dev(&hdr, p.hdr + env, sizeof(EnvHdr));
@@ -1459,10 +1379,8 @@ int get_state(libenv_env *handle, int env_idx, char *data, int length) {
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
     pg_fassert(env_idx >= 0 && env_idx < v->num_envs);
-    if (v->capturing())
+    if (!v->try_sync(true))  // wait_for_stepping_threads
         return -1;
-    v->ensure_initial_reset();
-    v->sync();  // wait_for_stepping_threads
     host::HostEnv e;
     fetch_env(v, env_idx, e);
     const GameVTable *g = v->games[(size_t)env_idx % v->games.size()];
@@ -1494,13 +1412,9 @@ void set_state(libenv_env *handle, int env_idx, char *data, int length) {
         pg_fatal("set_state: %s\n", ex.what());
     }
     store_env(v, env_idx, e);
-#ifndef PG_HOSTSIM
-    CUDA_CHECK(cudaDeviceSynchronize());  // the uploads ran on the legacy stream; the kernels below do not order against it
-#endif
+    device_sync();  // the uploads ran on the legacy stream; the kernels below do not order against it
     // Game::observe(): re-render this env and rewrite its rew / first / info slots from the restored step_data
-    KParams p = v->base;
-    p.assets = v->d_assets[gi];
-    p.game_id = g->id;
+    KParams p = v->game_params((int)gi);
     p.env_first = env_idx;
     p.env_step = 1;
     p.env_count = 1;
@@ -1534,13 +1448,12 @@ int pgb200_kernel_timing_begin(libenv_env *handle, int max_launch_pairs) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing() || v->base.level_end)
+    if (v->base.level_end || !v->try_sync())
         return -1;
-    v->sync();
     while ((int)v->tev_pool.size() < 4 * max_launch_pairs) {
         cudaEvent_t e;
         CUDA_CHECK(cudaEventCreate(&e));
-        v->tev_pool.push_back(e);
+        v->tev_pool.push_back(v->own(e));
     }
     v->tev_used = 0;
     v->tev_envs.clear();
@@ -1555,9 +1468,8 @@ int pgb200_kernel_timing_end(libenv_env *handle, double *out) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->capturing())
+    if (!v->try_sync())
         return -1;
-    v->sync();
     v->timing = false;
     double logic_ms = 0, setup_ms = 0, render_ms = 0, envs = 0;
     const int pairs = (int)(v->tev_used / 4);
