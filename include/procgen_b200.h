@@ -254,6 +254,32 @@ LIBENV_API int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out);
 LIBENV_API int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count, int capacity);
 LIBENV_API int pgb200_level_bank_info(libenv_env *handle, int *levels, int64_t *bytes);
 
+/* Level lookahead: each env's next level generated while its current episode plays. With num_levels = 0 (the
+ * unbounded level distribution) no bank can hold the levels, and an episode end generates its next level inside the
+ * step, on one warp, which sets the step's time for caveflyer, jumper and leaper. An env's next seed is known as
+ * soon as its episode starts (the next draw of its level seed generator), so a lookahead handle generates that
+ * level into a slot of its own beside the frames of the step, and the reset at the episode's end copies it.
+ * pgb200_enable_level_lookahead performs the initial reset if it has not happened yet, gives every env a slot sized
+ * by its own game (in the bank's slot layout: 24-77 KB, so about 5 GB for coinrun at 65 536 envs), generates each
+ * env's predicted next level into it and returns. A second call does nothing and returns 0; -1 (nothing changed)
+ * while the handle's stream is capturing. There is no off switch; the memory is released by libenv_close.
+ * At every reset inside a step the seed is chosen as always (game end, time limit, action -1, a next_level_seed
+ * override, the +997 of sequential levels). A bank that holds it serves the level; otherwise the env's slot does if
+ * it holds that seed for the env's options; otherwise the level is generated. Every output and every state byte,
+ * error bits and max_ents_seen included, is the one a handle without lookahead gives: its only effect is speed.
+ * After each such reset the env's next seed is predicted (its current seed while episodes_remaining != 0, else the
+ * next draw of its level seed generator) and generated into its slot unless a bank or the slot already holds it.
+ * A prediction can miss: an override, set_state, or a completed level of use_sequential_levels (+997; the draw is
+ * predicted) lead to a reset that generates. The initial reset, get_state / set_state, the wire format, override
+ * consumption, paused envs, final outputs, the consumer output and the bank are unaffected.
+ * CUDA graphs: a step captured after the call uses lookahead at every replay, one captured before it never does. A
+ * handle without lookahead runs the kernels it ran before.
+ * pgb200_level_lookahead_info: out[0] resets served from a lookahead slot, out[1] resets served from the bank,
+ * out[2] resets that generated (all three counted from the call on), out[3] the device bytes lookahead holds (slots
+ * and staging); all 0 without lookahead. Returns 0, or -1 while the handle's stream is capturing. */
+LIBENV_API int pgb200_enable_level_lookahead(libenv_env *handle);
+LIBENV_API int pgb200_level_lookahead_info(libenv_env *handle, int64_t *out /* [4] */);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -278,7 +304,8 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * launches issued, a captured step once, not its replays.
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
- * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank, pgb200_get_device_buffers
+ * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank,
+ * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, pgb200_get_device_buffers
  * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
  * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step

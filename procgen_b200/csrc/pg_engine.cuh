@@ -12,6 +12,8 @@
 // Expression types (float vs double, int promotion) are kept exactly as in the reference line
 // each function cites, because results must be bit-identical; see pg_common.cuh.
 #pragma once
+#include <type_traits>
+
 #include "pg_bank.cuh"
 
 namespace pg {
@@ -790,8 +792,9 @@ struct Engine {
     // level_seed_override >= 0 (pgb200_get_next_level_seeds) replaces the draw of the next level seed and
     // nothing else: level_seed_rand_gen is not advanced. Returns whether the override was taken.
     // BANK: a level the bank holds (bank_copy_level) is copied instead of generated; nothing else changes.
-    template <bool BANK = false>
-    static PG_HD bool reset(Ctx &c, int32_t level_seed_override = -1, const LevelBank *bank = nullptr) {
+    // Source (level lookahead): src->copy_level(c) decides instead whether the level is copied, and from where.
+    template <bool BANK = false, class Source = void>
+    static PG_HD bool reset(Ctx &c, int32_t level_seed_override = -1, const LevelBank *bank = nullptr, const Source *src = nullptr) {
         EnvHdr &h = *c.h;
         bool took = false;
         h.reset_count++;
@@ -810,7 +813,12 @@ struct Engine {
             h.done = 0;
             h.level_complete = 0;
         }
-        if (!BANK || !bank_copy_level<G>(c, *bank)) {
+        bool generate;
+        if constexpr (std::is_void<Source>::value)
+            generate = !BANK || !bank_copy_level<G>(c, *bank);
+        else
+            generate = !src->copy_level(c);
+        if (generate) {
             mt_seed(*c.rng, (uint32_t)h.current_level_seed);
             G::game_reset(c);
         }
@@ -851,12 +859,13 @@ struct Engine {
         h.prev_level_seed = h.current_level_seed;
         return h.done != 0;
     }
-    template <bool BANK = false>
-    static PG_HD bool step_finish(Ctx &c, bool do_reset, int32_t level_seed_override, const LevelBank *bank = nullptr) {
+    template <bool BANK = false, class Source = void>
+    static PG_HD bool step_finish(Ctx &c, bool do_reset, int32_t level_seed_override, const LevelBank *bank = nullptr,
+                                  const Source *src = nullptr) {
         EnvHdr &h = *c.h;
         bool took = false;
         if (do_reset)
-            took = reset<BANK>(c, level_seed_override, bank);
+            took = reset<BANK, Source>(c, level_seed_override, bank, src);
         if (h.options.use_sequential_levels && h.level_complete)
             h.done = 0;
         h.episode_done = h.done;

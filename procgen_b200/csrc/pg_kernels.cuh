@@ -70,6 +70,9 @@ struct KParams {
     // handle steps in two phases as with final outputs; without them, phase A's level_end goes to bank_level_end
     LevelBank bank;
     uint8_t *bank_level_end;    // [N] handle-owned
+    // optional level lookahead (pgb200_enable_level_lookahead); look.slot.slots null = off. The handle then steps in
+    // two phases as with a bank, and its phase B lists the envs whose next level the lookahead kernel generates
+    LevelLookahead look;
 };
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
@@ -223,15 +226,84 @@ PG_HD bool env_step_logic_final(const KParams &p, int env) {
     return do_reset;
 }
 
+// Where a lookahead handle's reset takes its level from: the bank where it holds the seed (BANK), else the env's
+// lookahead slot where it holds the seed for options like the env's, else generation. Counts the choice in
+// p.look.served.
+template <class G, bool BANK>
+struct LookaheadSource {
+    const KParams &p;
+    int env;
+    PG_HD bool copy_level(Ctx &c) const {
+        int from = 2;
+        if (BANK && bank_copy_level<G>(c, p.bank)) {
+            from = 1;
+        } else {
+            unsigned char *slot = lookahead_slot(p.look, env);
+            if (slot_key(slot) == c.h->current_level_seed && slot_usable(slot) != 0 && bank_options_match(c.h->options, p.look.slot.options)) {
+                bank_copy_slot<G>(c, slot, p.look.slot);
+                from = 0;
+            }
+        }
+#if defined(__CUDA_ARCH__)
+        if ((threadIdx.x & 31u) == 0)
+            atomicAdd(p.look.served + from, 1ull);
+#else
+        p.look.served[from]++;
+#endif
+        return from != 2;
+    }
+};
+
+// The level env's next reset is predicted to play: its current level again while episodes_remaining != 0, otherwise
+// the next draw of level_seed_rand_gen (a completed level of use_sequential_levels goes on by +997 instead, and
+// misses). Unless the bank holds it (`bank`) or the env's slot already does, the slot is keyed with the prediction,
+// marked not usable, and env is appended to p.look.list for the lookahead kernel. An env whose generator an older blob
+// left half-twisted, or whose options are not the handle's, keeps its slot as it is.
+PG_HD void lookahead_predict(const KParams &p, int env, bool bank) {
+    const EnvHdr &h = p.hdr[env];
+    int32_t seed = h.current_level_seed;
+    if (h.episodes_remaining == 0 && !rand_peek_randint(p.lvl_rng[env], h.level_seed_low, h.level_seed_high, &seed))
+        return;
+    if (!bank_options_match(h.options, p.look.slot.options))
+        return;
+    if (bank && bank_find(p.bank.seeds, *p.bank.count, seed) >= 0)
+        return;
+    unsigned char *slot = lookahead_slot(p.look, env);
+    if (slot_key(slot) == seed)
+        return;
+#if defined(__CUDA_ARCH__)
+    __syncwarp();
+    if ((threadIdx.x & 31u) == 0) {
+        slot_key(slot) = seed;
+        slot_usable(slot) = 0;
+        p.look.list[atomicAdd(p.look.count, 1u)] = env;
+    }
+    __syncwarp();
+#else
+    slot_key(slot) = seed;
+    slot_usable(slot) = 0;
+    p.look.list[(*p.look.count)++] = env;
+#endif
+}
+
 // Phase B: the rest of Game::step for an env whose level ended in phase A. The reset reads and consumes the
 // env's next_level_seed entry as env_step_logic<LEVEL_CHOICE> does; then Game::observe's camera and scalars.
 // BANK: the handle has a level bank, which the reset copies the level from when it holds it.
-template <class G, class Frame, bool BANK = false>
+// LOOK: the handle has level lookahead: the reset's level comes from LookaheadSource, and the env's next one is
+// predicted (lookahead_predict).
+template <class G, class Frame, bool BANK = false, bool LOOK = false>
 PG_HD void env_finish_logic(const KParams &p, int env) {
     Ctx c = make_ctx(p, env);
     const int32_t next_seed = p.next_level_seed ? p.next_level_seed[env] : -1;
-    if (Engine<G>::template step_finish<BANK>(c, true, next_seed, &p.bank))
-        p.next_level_seed[env] = -1;
+    if constexpr (LOOK) {
+        const LookaheadSource<G, BANK> src{p, env};
+        if (Engine<G>::template step_finish<BANK, const LookaheadSource<G, BANK>>(c, true, next_seed, &p.bank, &src))
+            p.next_level_seed[env] = -1;
+        lookahead_predict(p, env, BANK);
+    } else {
+        if (Engine<G>::template step_finish<BANK>(c, true, next_seed, &p.bank))
+            p.next_level_seed[env] = -1;
+    }
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, *c.h);
 }
@@ -243,12 +315,11 @@ PG_HD size_t bank_stage_bytes(const KParams &p) {
            sizeof(MT19937) + (((size_t)p.scratch_stride * sizeof(int32_t) + 15) & ~(size_t)15);
 }
 
-// Generates the level of bank.seeds[item] of the launch's game in `stage`, as a reset would from the state
-// init_constants leaves with the handle's options, then stores it in slot `item`, marked usable if it fits the
-// game's slot. One warp (or one thread in the host debug build).
-template <class G>
-PG_HD void bank_generate_level(const KParams &p, int item, unsigned char *stage) {
-    const LevelBank &b = p.bank;
+// Generates the level of `seed` of the launch's game in `stage`, as a reset would from the state init_constants
+// leaves with the handle's options, then stores it in the slot slot_of() returns (laid out as `b` describes), marked
+// usable if it fits the game's slot. One warp (or one thread in the host debug build).
+template <class G, class SlotOf>
+PG_HD void bank_generate_level(const KParams &p, const LevelBank &b, int32_t seed, SlotOf slot_of, unsigned char *stage) {
     Ctx c;
     c.h = reinterpret_cast<EnvHdr *>(stage);
     c.ents = reinterpret_cast<Entity *>(stage + sizeof(EnvHdr));
@@ -272,12 +343,12 @@ PG_HD void bank_generate_level(const KParams &p, int item, unsigned char *stage)
     h.fixed_asset_seed = p.fixed_asset_seed;
     h.level_seed_low = p.level_seed_low;
     h.level_seed_high = p.level_seed_high;
-    h.current_level_seed = b.seeds[item];
+    h.current_level_seed = seed;
     h.episodes_remaining = 1;
     ctx_refresh(c);
     mt_seed(*c.rng, (uint32_t)h.current_level_seed);
     G::game_reset(c);
-    unsigned char *slot = b.slots + (size_t)item * b.slot_bytes;
+    unsigned char *slot = slot_of();
     const bool usable = h.max_ents_seen <= G::ENT_CAP && h.grid_size <= G::GRID_CAP && h.agent_idx < c.ent_cap;
     if (usable) {
         bank_copy_vecs(slot + BANK_SLOT_HEAD, &h, (int)sizeof(EnvHdr));
@@ -291,6 +362,13 @@ PG_HD void bank_generate_level(const KParams &p, int item, unsigned char *stage)
         pg_warp_for(G::PERSIST_SCRATCH_WORDS, [=](int k) { ds[k] = ss[k]; });
     }
     *reinterpret_cast<int32_t *>(slot) = usable ? 1 : 0;  // every lane stores the same value
+}
+
+// The level p.look.list[item]'s slot is keyed with, generated into the slot (lookahead kernel, bulk fill)
+template <class G>
+PG_HD void lookahead_generate(const KParams &p, int item, unsigned char *stage) {
+    unsigned char *slot = lookahead_slot(p.look, p.look.list[item]);
+    bank_generate_level<G>(p, p.look.slot, slot_key(slot), [=] { return slot; }, stage);
 }
 
 // Profiling variant (-DPG_PHASE_TIMING): the setup kernel's phases, SM cycles of env's last frame in header slots

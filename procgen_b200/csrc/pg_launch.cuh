@@ -110,7 +110,9 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
 // Phase B of a step with final outputs: the resets of the envs phase A listed. Persistent and ticketed like the
 // logic kernel, because level generation runs here (milliseconds for caveflyer, jumper and leaper).
 // BANK: the handle has a level bank; the only kernel a banked step adds to those of an unbanked one.
-template <class G, bool BANK = false>
+// LOOK: the handle has level lookahead: resets copy from the env's lookahead slot where it holds their level, and list
+// the envs whose next level lookahead_kernel generates.
+template <class G, bool BANK = false, bool LOOK = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -124,10 +126,10 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_ker
             break;
         const int env = p.reset_list[t];
         // a banked step's reset runs here: its cycles join phase A's in the profiling aid
-        const long long t0 = (BANK && p.dbg_cycles) ? clock64() : 0;
-        env_finish_logic<G, Frame, BANK>(p, env);
+        const long long t0 = ((BANK || LOOK) && p.dbg_cycles) ? clock64() : 0;
+        env_finish_logic<G, Frame, BANK, LOOK>(p, env);
         __syncwarp();
-        if (BANK && p.dbg_cycles && lane == 0)
+        if ((BANK || LOOK) && p.dbg_cycles && lane == 0)
             p.dbg_cycles[env] += (uint32_t)(clock64() - t0);
     }
 }
@@ -140,9 +142,41 @@ __global__ void __launch_bounds__(kLogicThreads) bank_build_kernel(KParams p, un
     if (w >= warps)
         return;
     for (int item = w; item < count; item += warps) {
-        bank_generate_level<G>(p, item, stage + (size_t)w * bank_stage_bytes(p));
+        bank_generate_level<G>(p, p.bank, p.bank.seeds[item], [&] { return p.bank.slots + (size_t)item * p.bank.slot_bytes; },
+                               stage + (size_t)w * bank_stage_bytes(p));
         __syncwarp();
     }
+}
+
+// Level lookahead: the levels of the envs p.look.list holds (count[0] of them), generated into their slots. Persistent
+// with a fixed grid of p.look.stage_warps warps, each with its own staging area, ticketed over the list by count[1];
+// the count is read on the device, so a step that launches it stays capturable.
+template <class G>
+__global__ void __launch_bounds__(kLogicThreads) lookahead_kernel(KParams p, unsigned int *count) {
+    const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (w >= p.look.stage_warps)
+        return;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned n = count[0];
+    unsigned char *stage = p.look.stage + (size_t)w * bank_stage_bytes(p);
+    while (true) {
+        unsigned t = 0;
+        if (lane == 0)
+            t = atomicAdd(count + 1, 1u);
+        t = __shfl_sync(0xffffffffu, t, 0);
+        if (t >= n)
+            break;
+        lookahead_generate<G>(p, (int)t, stage);
+        __syncwarp();
+    }
+}
+
+// Level lookahead's bulk fill: one warp per env of the launch predicts its next level (lookahead_predict)
+template <class G>
+__global__ void __launch_bounds__(kLogicThreads) lookahead_predict_kernel(KParams p) {
+    const int i = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (i < p.env_count)
+        lookahead_predict(p, p.env_first + i * p.env_step, p.bank.slots != nullptr);
 }
 
 // Frame setup: one warp per env (4 envs per block). Everything about a frame that is O(entities +
@@ -460,8 +494,10 @@ struct LaunchCtx {
     int render_smem_floor;    // dynamic shared memory requested per render CTA is at least this (co-residency knob)
     Event *tev;               // optional: 4 events (before logic, after it, after setup, after render) for kernel timing
     // work counter of this launch slot (one per in-flight logic kernel); a two-phase step keeps its list's count and
-    // phase B's ticket in the next two words
+    // phase B's ticket in the next two words, and level lookahead its list's count and ticket in the two after them
     unsigned int *ticket;
+    Stream look_stream;       // level lookahead: the side stream the launch's lookahead kernel runs on, forked at
+    Event look_fork;          // look_fork behind phase B (the runtime joins it back behind the launch's last work)
     int64_t *launch_counter;
 };
 
@@ -511,11 +547,11 @@ static inline int logic_grid(const KParams &p, const LaunchCtx &lc) {
 
 // logic: clears the launch's ticket, then runs the logic kernel over the launch's envs. FINAL: phase A of a two-phase
 // step, which lists the envs whose level ends in p.reset_list and clears the list's count and phase B's ticket with
-// its own. A two-phase step stays on lc.stream: a priority-split logic stream would let the next launch that shares
+// its own (LOOK: and the lookahead list's count and ticket). A two-phase step stays on lc.stream: a priority-split logic stream would let the next launch that shares
 // this ticket slot clear it under phase B. A one-phase step's logic kernel may go to that stream (PGB200_PRIORITY_SPLIT).
-template <class G, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE>
+template <class G, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE, bool LOOK = false>
 void logic_phase(const KParams &p, const LaunchCtx &lc) {
-    constexpr size_t kTicketBytes = (FINAL ? 3 : 1) * sizeof(unsigned int);
+    constexpr size_t kTicketBytes = (LOOK ? 5 : FINAL ? 3 : 1) * sizeof(unsigned int);
 #ifndef PG_HOSTSIM
     const cudaStream_t ls = !FINAL && lc.logic_stream ? lc.logic_stream : lc.stream;
     CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, kTicketBytes, ls));
@@ -545,16 +581,32 @@ void logic_phase(const KParams &p, const LaunchCtx &lc) {
 }
 
 // finish: phase B's resets, the finish kernel over the envs phase A listed. BANK: they copy their levels from the
-// bank where it holds them.
-template <class G, bool BANK>
+// bank where it holds them. LOOK: or from their lookahead slots, and list the envs whose next level is to be generated.
+template <class G, bool BANK, bool LOOK = false>
 void finish_phase(const KParams &p, const LaunchCtx &lc) {
 #ifndef PG_HOSTSIM
-    finish_kernel<G, BANK><<<logic_grid(p, lc), kLogicThreads, 0, lc.stream>>>(p, lc.ticket + 2);
+    finish_kernel<G, BANK, LOOK><<<logic_grid(p, lc), kLogicThreads, 0, lc.stream>>>(p, lc.ticket + 2);
     CUDA_CHECK(cudaGetLastError());
 #else
     (void)lc;
     using Frame = typename FrameFor<G>::type;
-    for (unsigned int j = 0; j < *p.reset_count; j++) env_finish_logic<G, Frame, BANK>(p, p.reset_list[j]);
+    for (unsigned int j = 0; j < *p.reset_count; j++) env_finish_logic<G, Frame, BANK, LOOK>(p, p.reset_list[j]);
+#endif
+}
+
+// lookahead: the lookahead kernel over the envs phase B listed, on the launch's side stream forked here, so that it
+// runs beside the frames phase (the runtime joins it back). The host debug build runs it in place, before the frames.
+template <class G>
+void lookahead_phase(const KParams &p, const LaunchCtx &lc) {
+#ifndef PG_HOSTSIM
+    CUDA_CHECK(cudaEventRecord(lc.look_fork, lc.stream));
+    CUDA_CHECK(cudaStreamWaitEvent(lc.look_stream, lc.look_fork, 0));
+    const int blocks = (p.look.stage_warps + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
+    lookahead_kernel<G><<<blocks, kLogicThreads, 0, lc.look_stream>>>(p, p.look.count);
+    CUDA_CHECK(cudaGetLastError());
+#else
+    (void)lc;
+    for (unsigned int j = 0; j < *p.look.count; j++) lookahead_generate<G>(p, (int)j, p.look.stage);
 #endif
 }
 
@@ -602,34 +654,41 @@ void frames_phase(const KParams &p, const LaunchCtx &lc) {
 //   initial reset, plain step                logic, frames(0)
 //   level bank, without final outputs        logic (phase A), finish, frames(0)
 //   final outputs, with or without a bank    logic (phase A), frames(1), finish, frames(2)
+// LOOK (level lookahead) takes the two-phase shape of a bank and runs the lookahead phase right behind the finish
+// phase, beside the frames that follow it.
 // A final-outputs step's phase A renders the final frames of the envs whose level ends, to final_rgb; phase B renders
 // the first frames of their next levels. A banked step without final outputs also runs its resets in the finish
 // kernel, so that its logic kernel is one that steps always run (its stack frame and registers stay those of the
 // step, which must fit the push_obj / sub_step recursion); phase A's level_end goes to the handle's bank_level_end.
 // PAUSE: the instantiations that skip the envs the handle's pause mask holds still; phase B, which only sees the
 // list, needs none.
-template <class G, int VIEW, bool INIT, bool PAUSE, bool FINAL, bool BANK>
+template <class G, int VIEW, bool INIT, bool PAUSE, bool FINAL, bool BANK, bool LOOK = false>
 void launch_step(const KParams &p, const LaunchCtx &lc) {
     KParams q = p;  // what the phases of a two-phase step see
     q.reset_count = lc.ticket + 1;
-    if constexpr (BANK && !FINAL)
+    q.look.count = lc.ticket + 3;
+    if constexpr ((BANK || LOOK) && !FINAL)
         q.level_end = p.bank_level_end;
-    if constexpr (FINAL || BANK)
-        logic_phase<G, false, false, true, PAUSE>(q, lc);
+    if constexpr (FINAL || BANK || LOOK)
+        logic_phase<G, false, false, true, PAUSE, LOOK>(q, lc);
     else if (!INIT && p.next_level_seed)
         logic_phase<G, false, true, false, PAUSE>(p, lc);
     else
         logic_phase<G, INIT, false, false, PAUSE>(p, lc);
     if constexpr (FINAL) {
         frames_phase<G, VIEW, 1, PAUSE>(q, lc);
-        finish_phase<G, BANK>(q, lc);
+        finish_phase<G, BANK, LOOK>(q, lc);
+        if constexpr (LOOK)
+            lookahead_phase<G>(q, lc);
         frames_phase<G, VIEW, 2, false>(q, lc);
     } else {
-        if constexpr (BANK)
-            finish_phase<G, true>(q, lc);
+        if constexpr (BANK || LOOK)
+            finish_phase<G, BANK, LOOK>(q, lc);
+        if constexpr (LOOK)
+            lookahead_phase<G>(q, lc);
         frames_phase<G, VIEW, 0, PAUSE>(p, lc);
     }
-    (*lc.launch_counter) += FINAL ? 6 : BANK ? 4 : 3;
+    (*lc.launch_counter) += (FINAL ? 6 : BANK || LOOK ? 4 : 3) + (LOOK ? 1 : 0);
 }
 
 template <class G, bool INIT, int VIEW>
@@ -640,8 +699,9 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
         launch_step<G, VIEW, true, false, false, false>(p, lc);
         return;
     }
-    // a handle without a pause mask, final outputs or a level bank runs exactly the kernels it ran before they existed
-    switch ((p.pause ? 1 : 0) | (p.level_end ? 2 : 0) | (p.bank.slots ? 4 : 0)) {
+    // a handle without a pause mask, final outputs, a level bank or level lookahead runs exactly the kernels it ran
+    // before they existed
+    switch ((p.pause ? 1 : 0) | (p.level_end ? 2 : 0) | (p.bank.slots ? 4 : 0) | (p.look.slot.slots ? 8 : 0)) {
     case 0: launch_step<G, VIEW, false, false, false, false>(p, lc); break;
     case 1: launch_step<G, VIEW, false, true, false, false>(p, lc); break;
     case 2: launch_step<G, VIEW, false, false, true, false>(p, lc); break;
@@ -650,6 +710,14 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
     case 5: launch_step<G, VIEW, false, true, false, true>(p, lc); break;
     case 6: launch_step<G, VIEW, false, false, true, true>(p, lc); break;
     case 7: launch_step<G, VIEW, false, true, true, true>(p, lc); break;
+    case 8: launch_step<G, VIEW, false, false, false, false, true>(p, lc); break;
+    case 9: launch_step<G, VIEW, false, true, false, false, true>(p, lc); break;
+    case 10: launch_step<G, VIEW, false, false, true, false, true>(p, lc); break;
+    case 11: launch_step<G, VIEW, false, true, true, false, true>(p, lc); break;
+    case 12: launch_step<G, VIEW, false, false, false, true, true>(p, lc); break;
+    case 13: launch_step<G, VIEW, false, true, false, true, true>(p, lc); break;
+    case 14: launch_step<G, VIEW, false, false, true, true, true>(p, lc); break;
+    case 15: launch_step<G, VIEW, false, true, true, true, true>(p, lc); break;
     }
 }
 
@@ -686,7 +754,28 @@ void launch_bank_build(const KParams &p, const LaunchCtx &lc, unsigned char *sta
 #else
     (void)lc;
     (void)warps;
-    for (int item = 0; item < count; item++) bank_generate_level<G>(p, item, stage);
+    for (int item = 0; item < count; item++)
+        bank_generate_level<G>(p, p.bank, p.bank.seeds[item], [&] { return p.bank.slots + (size_t)item * p.bank.slot_bytes; }, stage);
+#endif
+}
+
+// Level lookahead's bulk fill of the launch's envs: every env's next level predicted, then the listed ones generated
+// by p.look.stage_warps warps with staging at p.look.stage, on the launch's stream. p.look.count: two words, zero.
+template <class G>
+void launch_lookahead_fill(const KParams &p, const LaunchCtx &lc) {
+    if (p.env_count <= 0)
+        return;
+#ifndef PG_HOSTSIM
+    lookahead_predict_kernel<G><<<(p.env_count + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock, kLogicThreads, 0, lc.stream>>>(p);
+    CUDA_CHECK(cudaGetLastError());
+    const int blocks = (p.look.stage_warps + kLogicEnvsPerBlock - 1) / kLogicEnvsPerBlock;
+    lookahead_kernel<G><<<blocks, kLogicThreads, 0, lc.stream>>>(p, p.look.count);
+    CUDA_CHECK(cudaGetLastError());
+    (*lc.launch_counter) += 2;
+#else
+    (void)lc;
+    for (int i = 0; i < p.env_count; i++) lookahead_predict(p, p.env_first + i * p.env_step, p.bank.slots != nullptr);
+    for (unsigned int j = 0; j < *p.look.count; j++) lookahead_generate<G>(p, (int)j, p.look.stage);
 #endif
 }
 
@@ -705,6 +794,7 @@ struct GameVTable {
     void (*step[2])(const KParams &, const LaunchCtx &);
     void (*observe_only[2])(const KParams &, const LaunchCtx &);
     void (*bank_build)(const KParams &, const LaunchCtx &, unsigned char *, int, int);
+    void (*lookahead_fill)(const KParams &, const LaunchCtx &);
     int persist_scratch_words;  // G::PERSIST_SCRATCH_WORDS
 };
 
@@ -734,6 +824,7 @@ GameVTable make_vtable(int id) {
     vt.scratch_words = G::SCRATCH_WORDS;
     vt.persist_scratch_words = G::PERSIST_SCRATCH_WORDS;
     vt.bank_build = &launch_bank_build<G>;
+    vt.lookahead_fill = &launch_lookahead_fill<G>;
     vt.rot_records = FrameFor<G>::type::kMaxRot;
     vt.blit_records = FrameFor<G>::type::kMaxList;
     fill_view<G, G::MAX_VIEW_CELLS>(vt, 0);

@@ -95,6 +95,11 @@ static inline void stream_destroy(Stream s) { cudaStreamDestroy(s); }
 static inline void event_destroy(Event e) { cudaEventDestroy(e); }
 // on the legacy default stream, complete when they return
 static inline void dev_memset(void *dst, int value, size_t bytes) { CUDA_CHECK(cudaMemset(dst, value, bytes)); }
+// `rows` runs of `bytes` bytes, `pitch` bytes apart
+static inline void memset_strided(void *dst, int value, size_t bytes, size_t pitch, size_t rows) {
+    if (rows)
+        CUDA_CHECK(cudaMemset2D(dst, pitch, value, bytes, rows));
+}
 static inline void copy_to_dev(void *dst, const void *src, size_t bytes) { CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); }
 static inline void copy_from_dev(void *dst, const void *src, size_t bytes) { CUDA_CHECK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); }
 // on stream s, behind the work issued there before
@@ -130,6 +135,9 @@ static inline void host_unregister(void *) {}
 static inline void stream_destroy(Stream) {}
 static inline void event_destroy(Event) {}
 static inline void dev_memset(void *dst, int value, size_t bytes) { memset(dst, value, bytes); }
+static inline void memset_strided(void *dst, int value, size_t bytes, size_t pitch, size_t rows) {
+    for (size_t r = 0; r < rows; r++) memset((unsigned char *)dst + r * pitch, value, bytes);
+}
 static inline void copy_to_dev(void *dst, const void *src, size_t bytes) { memcpy(dst, src, bytes); }
 static inline void copy_from_dev(void *dst, const void *src, size_t bytes) { memcpy(dst, src, bytes); }
 static inline void copy_to_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
@@ -219,6 +227,19 @@ const GameVTable *find_game(const std::string &name) {
     return nullptr;
 }
 
+// The bank's slot layout of game g (pg_bank.cuh), for levels generated with `options`: int32 usable, int32 key (16 B) |
+// EnvHdr | Entity[ENT_CAP] | grid[GRID_CAP] | MT19937 | persistent scratch. Bank slots and lookahead slots share it.
+LevelBank slot_layout(const GameVTable *g, const Options &options) {
+    LevelBank b{};
+    b.ents_off = BANK_SLOT_HEAD + (int)sizeof(EnvHdr);
+    b.grid_off = b.ents_off + g->ent_cap * (int)sizeof(Entity);
+    b.rng_off = b.grid_off + ((g->grid_cap * (int)sizeof(int16_t) + 15) & ~15);
+    b.scratch_off = b.rng_off + (int)sizeof(MT19937);
+    b.slot_bytes = b.scratch_off + ((g->persist_scratch_words * (int)sizeof(int32_t) + 15) & ~15);
+    b.options = options;
+    return b;
+}
+
 // vecgame.cpp:156-167: system-independent hash of the game name
 static int32_t fnv1a(const char *str) {
     uint32_t hash = 0x811c9dc5u;
@@ -279,6 +300,16 @@ struct VecEnv {
     int bank_capacity = 0;
     int bank_levels = 0;
     int64_t bank_bytes = 0;
+    // allocated by pgb200_enable_level_lookahead: one slot per env in the bank's layout of its game (looks[g], one
+    // allocation at base.look.slot.slots), the list the finish kernels fill and its per-step staging: look_warps warps
+    // per side stream, one side stream (look_side, forked at look_fork and joined at look_join) per auxiliary stream
+    std::vector<LevelLookahead> looks;
+    int look_warps = 0;
+    size_t look_stage_bytes = 0;             // per side stream
+    unsigned long long *d_look_served = nullptr;
+    int64_t look_bytes = 0;
+    Stream look_side[PG_AUX_STREAMS] = {};
+    Event look_fork[PG_AUX_STREAMS] = {}, look_join[PG_AUX_STREAMS] = {};
     bool initial_reset_done = false;
     int64_t launches = 0;
     host::ConstGameFields const_fields;  // options Game::serialize writes but no kernel reads
@@ -309,8 +340,9 @@ struct VecEnv {
     int force_chunks = 0;            // measurement knobs (pgb200_set_launch_shape)
     bool serialize_launches = false;
     static constexpr int kMaxTickets = 64;   // launch slots in flight
-    // words per slot: the logic kernel's ticket; with final outputs also the pending-reset count and phase B's ticket
-    static constexpr int kTicketWords = 4;
+    // words per slot: the logic kernel's ticket; with final outputs also the pending-reset count and phase B's ticket;
+    // with level lookahead also its list's count and the lookahead kernel's ticket
+    static constexpr int kTicketWords = 8;
     unsigned int *d_tickets = nullptr;
     int max_logic_blocks = 1;        // logic blocks the device holds at once (device setup); the host build runs one env at a time
     int num_sms = 1;
@@ -387,11 +419,14 @@ struct VecEnv {
         lc.tev = nullptr;
         lc.ticket = d_tickets;
         lc.launch_counter = &launches;
+        lc.look_stream = nullptr;
+        lc.look_fork = nullptr;
         return lc;
     }
 
     // `base` as the launches of joint game g see it: the game's assets, id and fixed asset seed, and its slots of the
-    // level bank if there is one. The caller sets the launch's env range.
+    // level bank and of level lookahead where they exist. The caller sets the launch's env range (and, for lookahead,
+    // the launch's segment of the list and its staging).
     KParams game_params(int g) const {
         KParams p = base;
         p.assets = d_assets[g];
@@ -399,6 +434,8 @@ struct VecEnv {
         p.fixed_asset_seed = fnv1a(games[g]->name);
         if (base.bank.slots)
             p.bank = banks[g];
+        if (base.look.slot.slots)
+            p.look.slot = looks[g].slot;
         return p;
     }
 
@@ -451,6 +488,14 @@ struct VecEnv {
                     p.reset_list = base.reset_list + g * per_game + lo;  // the launch's own segment
                 LaunchCtx lc = lctx();
                 lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
+                if (base.look.slot.slots) {
+                    // launches that share a side stream run their lookahead kernels one after the other
+                    const int side = k % kAuxStreams;
+                    p.look.list = base.look.list + g * per_game + lo;
+                    p.look.stage = base.look.stage + side * look_stage_bytes;
+                    lc.look_stream = look_side[side];
+                    lc.look_fork = look_fork[side];
+                }
                 if (nstreams) {
                     lc.stream = aux[k % nstreams];
                     if (priority_split) {
@@ -490,6 +535,12 @@ struct VecEnv {
                     CUDA_CHECK(cudaMemcpyAsync(rgb_dst + (size_t)lo * frame, base.rgb + (size_t)lo * frame, (size_t)(hi - lo) * frame,
                                                cudaMemcpyDeviceToHost, lc.stream));
                     rgb_copy_enqueued = true;
+                }
+                // the lookahead kernel joins the launch's stream behind everything above, which never waits for it;
+                // the step still ends with it, so that a captured step is self-contained
+                if (!init && lc.look_stream && hi > lo) {
+                    CUDA_CHECK(cudaEventRecord(look_join[k % kAuxStreams], lc.look_stream));
+                    CUDA_CHECK(cudaStreamWaitEvent(lc.stream, look_join[k % kAuxStreams], 0));
                 }
 #endif
             }
@@ -1126,16 +1177,9 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
         // a banked step lists its resets as a step with final outputs does (launch_step)
         v->opt_in_array(base.bank_level_end, 1, 0);
         v->opt_in_array(base.reset_list, 1, 0);
-        // per game: int32 usable (16 B) | EnvHdr | Entity[ENT_CAP] | grid[GRID_CAP] | MT19937 | persistent scratch
         size_t total = 0;
         for (const GameVTable *g : v->games) {
-            LevelBank b{};
-            b.ents_off = BANK_SLOT_HEAD + (int)sizeof(EnvHdr);
-            b.grid_off = b.ents_off + g->ent_cap * (int)sizeof(Entity);
-            b.rng_off = b.grid_off + ((g->grid_cap * (int)sizeof(int16_t) + 15) & ~15);
-            b.scratch_off = b.rng_off + (int)sizeof(MT19937);
-            b.slot_bytes = b.scratch_off + ((g->persist_scratch_words * (int)sizeof(int32_t) + 15) & ~15);
-            b.options = base.options;
+            LevelBank b = slot_layout(g, base.options);
             b.seeds = v->d_bank_seeds;
             b.count = v->d_bank_count;
             b.slots = reinterpret_cast<unsigned char *>(total);  // offset until the allocation below
@@ -1166,6 +1210,105 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
     copy_to_dev_async(v->d_bank_count, &n_dev, sizeof(int32_t), v->stream);
     v->sync();  // the host sources above, then the staging
     v->bank_levels = n;
+    return 0;
+}
+
+int pgb200_enable_level_lookahead(libenv_env *handle) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    KParams &base = v->base;
+    if (base.look.slot.slots)
+        return 0;
+    if (!v->begin_opt_in(false))  // the fill waits for the device, so it never runs under capture
+        return -1;
+    const int G = (int)v->games.size();
+    const int per_game = v->num_envs / G;
+    // a lookahead handle lists its resets as a banked one does (launch_step)
+    v->opt_in_array(base.bank_level_end, 1, 0);
+    v->opt_in_array(base.reset_list, 1, 0);
+    v->opt_in_array(base.look.list, 1, 0);
+    size_t total = 0;
+    for (const GameVTable *g : v->games) {
+        LevelLookahead l{};
+        l.slot = slot_layout(g, base.options);
+        l.slot.slots = reinterpret_cast<unsigned char *>(total);  // offset until the allocation below
+        total += (size_t)per_game * l.slot.slot_bytes;
+        v->looks.push_back(l);
+    }
+    unsigned char *slots = v->alloc<unsigned char>(total);
+    for (LevelLookahead &l : v->looks) {
+        l.slot.slots = slots + reinterpret_cast<size_t>(l.slot.slots);
+        memset_strided(l.slot.slots + sizeof(int32_t), 0xff, sizeof(int32_t), (size_t)l.slot.slot_bytes, (size_t)per_game);  // keys -1
+    }
+    // per-step staging: as many warps per side stream as a quarter of the bank build's budget allows, at most what
+    // a launch's resets need at once
+    const size_t stage_bytes = bank_stage_bytes(base);
+    v->look_warps = (int)std::min<size_t>(std::max<size_t>(((size_t)64 << 20) / ((size_t)VecEnv::kAuxStreams * stage_bytes), 1), 128);
+    v->look_warps = std::min(v->look_warps, v->max_logic_blocks * kLogicEnvsPerBlock);
+    v->look_stage_bytes = (size_t)v->look_warps * stage_bytes;
+    unsigned char *step_stage = v->alloc<unsigned char>(VecEnv::kAuxStreams * v->look_stage_bytes);
+    v->d_look_served = v->alloc<unsigned long long>(3);
+    v->look_bytes = (int64_t)total + (int64_t)(VecEnv::kAuxStreams * v->look_stage_bytes) + (int64_t)v->num_envs * (int64_t)sizeof(int32_t) +
+                    3 * (int64_t)sizeof(unsigned long long);
+#ifndef PG_HOSTSIM
+    // The side streams the lookahead kernels run on beside the frames. Render CTAs fill the SMs, and a stream's
+    // priority decides whose pending blocks are placed first: at high priority the generation warps start as soon as
+    // a slot frees, and the step (which ends with them) is faster than at low priority (DESIGN §7).
+    int prio_lo = 0, prio_hi = 0;
+    CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+    const int prio = prio_hi;
+    for (int s = 0; s < VecEnv::kAuxStreams; s++) {
+        cudaStream_t st = nullptr;
+        CUDA_CHECK(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio));
+        v->look_side[s] = v->own(st);
+        cudaEvent_t e[2];
+        for (cudaEvent_t &ev : e) {
+            CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+            v->own(ev);
+        }
+        v->look_fork[s] = e[0];
+        v->look_join[s] = e[1];
+    }
+#endif
+    device_sync();  // alloc's memsets ran on the legacy stream
+    base.look.games = G;
+    base.look.stage = step_stage;
+    base.look.stage_warps = v->look_warps;
+    base.look.served = v->d_look_served;
+    // the bulk fill: every env's next level predicted, then generated with the bank build's staging budget
+    int warps = (int)std::min<size_t>((size_t)std::max(per_game, 1), std::max<size_t>(((size_t)256 << 20) / stage_bytes, 1));
+    warps = std::min(warps, v->max_logic_blocks * kLogicEnvsPerBlock);
+    std::unique_ptr<unsigned char, void (*)(void *)> stage((unsigned char *)dev_malloc((size_t)warps * stage_bytes), dev_free);
+    for (int g = 0; g < G; g++) {
+        KParams p = v->game_params(g);
+        p.look.slot = v->looks[g].slot;
+        p.env_first = g;
+        p.env_step = G;
+        p.env_count = per_game;
+        p.look.list = base.look.list + g * per_game;
+        p.look.count = v->d_tickets;  // the list's count and the lookahead kernel's ticket
+        p.look.stage = stage.get();
+        p.look.stage_warps = warps;
+        memset_async(v->d_tickets, 0, 2 * sizeof(unsigned int), v->stream);
+        LaunchCtx lc = v->lctx();
+        v->games[g]->lookahead_fill(p, lc);
+    }
+    v->sync();  // then the staging is released
+    base.look.slot = v->looks[0].slot;  // last: a non-null slots pointer is what selects the lookahead kernels
+    return 0;
+}
+
+int pgb200_level_lookahead_info(libenv_env *handle, int64_t *out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    unsigned long long served[3] = {0, 0, 0};
+    if (v->d_look_served) {
+        if (!v->try_sync())
+            return -1;
+        copy_from_dev(served, v->d_look_served, sizeof(served));
+    }
+    for (int i = 0; i < 3; i++) out[i] = (int64_t)served[i];
+    out[3] = v->look_bytes;
     return 0;
 }
 

@@ -450,6 +450,34 @@ class BaseProcgenEnv:
         self._lib.pgb200_level_bank_info(self._h, C.byref(levels), C.byref(nbytes))
         return {"levels": levels.value, "bytes": nbytes.value}
 
+    def enable_level_lookahead(self) -> None:
+        """Generate each env's next level while its current episode plays (level lookahead), for num_levels = 0 and
+        any other level set a bank does not hold: an env's next seed is known when its episode starts, so its level is
+        generated into a slot of its own beside the frames of a step, and the reset at the episode's end copies it
+        instead of generating it inside the step. Only speed changes: every output and state is the one a handle
+        without lookahead gives. A prediction can miss (next_level_seeds() overrides, set_state, a completed level of
+        use_sequential_levels): that reset generates as before. A bank, where there is one, serves its seeds first.
+
+        Memory: one slot per env, sized by its game (24-77 KB; about 5 GB for coinrun at 65 536 envs), and staging,
+        held until close(); level_lookahead_info()["bytes"] reports it. There is no off switch. The call generates every
+        env's next level before it returns; a second call does nothing. CUDA graphs captured after it use lookahead,
+        ones captured before it never do."""
+        self._refuse_in_capture("enable_level_lookahead")
+        self._wait_for_replays()
+        if self._lib.pgb200_enable_level_lookahead(self._h) != 0:
+            raise RuntimeError("pgb200_enable_level_lookahead failed")
+
+    def level_lookahead_info(self) -> dict:
+        """{"served": resets served from a lookahead slot, "bank": resets served from the bank, "generated": resets
+        that generated their level (the three counted from enable_level_lookahead() on), "bytes": device memory
+        lookahead holds}; zeros without lookahead."""
+        self._refuse_in_capture("level_lookahead_info")
+        self._wait_for_replays()
+        out = (C.c_int64 * 4)()
+        if self._lib.pgb200_level_lookahead_info(self._h, out) != 0:
+            raise RuntimeError("pgb200_level_lookahead_info failed")
+        return dict(zip(("served", "bank", "generated", "bytes"), list(out)))
+
     def callmethod(self, method: str, *args, **kwargs):
         return getattr(self, method)(*args, **kwargs)
 

@@ -58,7 +58,8 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_frame_info", "pgb200_set_rgb_mirror", "pgb200_mirror_parity",
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
            "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
-           "pgb200_build_level_bank", "pgb200_level_bank_info"]
+           "pgb200_build_level_bank", "pgb200_level_bank_info", "pgb200_enable_level_lookahead",
+           "pgb200_level_lookahead_info"]
 
 _lib = None
 
@@ -86,6 +87,10 @@ def bind(lib):
     lib.pgb200_build_level_bank.restype = C.c_int
     lib.pgb200_level_bank_info.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int64)]
     lib.pgb200_level_bank_info.restype = C.c_int
+    lib.pgb200_enable_level_lookahead.argtypes = [C.c_void_p]
+    lib.pgb200_enable_level_lookahead.restype = C.c_int
+    lib.pgb200_level_lookahead_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+    lib.pgb200_level_lookahead_info.restype = C.c_int
     lib.pgb200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     lib.pgb200_set_stream.restype = None
     lib.pgb200_get_errors.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
