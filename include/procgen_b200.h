@@ -280,6 +280,38 @@ LIBENV_API int pgb200_level_bank_info(libenv_env *handle, int *levels, int64_t *
 LIBENV_API int pgb200_enable_level_lookahead(libenv_env *handle);
 LIBENV_API int pgb200_level_lookahead_info(libenv_env *handle, int64_t *out /* [4] */);
 
+/* Rollout: every step also stores its rgb, rew and first into a ring of `slots` slots, so that a learner's rollout
+ * storage is filled by the render kernel itself instead of by a copy of the outputs after each step (the next step
+ * overwrites them). The arrays are slot-major, so rgb + t * num_envs * 12288 is one contiguous [num_envs][64][64][3]
+ * block, the shape of a learner's obs_buf[t]:
+ *   rgb    [slots][num_envs][64][64][3]  uint8
+ *   rew    [slots][num_envs]             float
+ *   first  [slots][num_envs]             uint8
+ *   cursor [1]                           int32, the slot the latest step (or the first call) wrote
+ * They are handle-owned device memory (host memory in the CPU debug build), valid until libenv_close, which frees
+ * them; there is no off switch. The first call performs the initial reset if it has not happened yet, allocates the
+ * arrays, writes the current rgb, rew and first into slot 0, sets *cursor = 0, waits and returns 0. A later call with
+ * the same `slots` returns the same pointers. Returns -1 (nothing changed) when slots < 2, when the ring's byte size
+ * overflows, when a later call asks for a different `slots`, or for the first call while the handle's stream is
+ * capturing.
+ * The invariant: after every step, *cursor has moved from c to c' = (c + 1) % slots and slot c' holds exactly that
+ * step's rgb, rew and first, byte for byte. Nothing else any step outputs changes. So with final outputs the slot
+ * holds the first frame of the next level (what rgb holds), not the final frame; a paused env's slot holds the frame
+ * it is paused on with rew = 0 and first = 0. Every launch shape, joint game list and view, and host-buffer handles
+ * follow it (there the arrays are complete once libenv_observe returns). get_state / set_state and
+ * pgb200_set_consumer_output neither read nor write the rollout.
+ * The cursor advances on the device, on the handle's stream, ahead of the step's render kernels: a step captured in
+ * a CUDA graph after the first call fills successive slots at every replay; one captured before it never writes the
+ * rollout. A handle without a rollout runs the kernels it ran before. A rollout of T steps plus the observation to
+ * bootstrap from needs slots >= T + 1. */
+struct pgb200_rollout {
+    uint8_t *rgb;     /* [slots][num_envs][64][64][3] */
+    float *rew;       /* [slots][num_envs] */
+    uint8_t *first;   /* [slots][num_envs] */
+    int32_t *cursor;  /* [1]: the slot the latest step (or the first call) wrote */
+};
+LIBENV_API int pgb200_get_rollout(libenv_env *handle, int slots, struct pgb200_rollout *out);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -305,7 +337,7 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
  * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank,
- * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, pgb200_get_device_buffers
+ * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, the first pgb200_get_rollout, pgb200_get_device_buffers
  * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
  * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step

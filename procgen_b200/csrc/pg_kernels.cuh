@@ -6,6 +6,16 @@
 
 namespace pg {
 
+// A handle's rollout (pgb200_get_rollout): `slots` copies of the step outputs rgb, rew and first, slot-major
+struct Rollout {
+    uint8_t *rgb;      // [slots][num_envs][64][64][3]
+    float *rew;        // [slots][num_envs]
+    uint8_t *first;    // [slots][num_envs]
+    int32_t *cursor;   // [1] the slot the current step writes (device)
+    int32_t slots;
+    int32_t num_envs;  // the handle's, not the launch's
+};
+
 struct KParams {
     // state (HBM)
     EnvHdr *hdr;
@@ -73,7 +83,21 @@ struct KParams {
     // optional level lookahead (pgb200_enable_level_lookahead); look.slot.slots null = off. The handle then steps in
     // two phases as with a bank, and its phase B lists the envs whose next level the lookahead kernel generates
     LevelLookahead look;
+    // optional rollout (pgb200_get_rollout); roll.rgb null = off. Every step also stores each env's rgb, rew and first
+    // into slot *roll.cursor of the ring, which the step advances on the device before its render kernels
+    Rollout roll;
 };
+
+// Where env's outputs of the current step go in the rollout: slot *roll.cursor, slot-major
+PG_HD size_t rollout_index(const KParams &p, int env) { return (size_t)*p.roll.cursor * (size_t)p.roll.num_envs + (size_t)env; }
+
+// The rollout's copy of env's scalar outputs of this step, which the logic or finish kernel has written by the time a
+// frame of the step is rendered
+PG_HD void rollout_store_scalars(const KParams &p, int env) {
+    const size_t i = rollout_index(p, env);
+    p.roll.rew[i] = p.rew[env];
+    p.roll.first[i] = p.first[env];
+}
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
     Ctx c;

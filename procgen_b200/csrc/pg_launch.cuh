@@ -282,9 +282,12 @@ __device__ __forceinline__ void pg_bulk_load(void *dst_smem, const void *src_gme
                  "l"(src_gmem), "r"(bytes), "r"(pg_smem_addr(bar))
                  : "memory");
 }
-// shared -> global; returns once the engine has read the source (the CTA may then exit / reuse it)
-__device__ __forceinline__ void pg_bulk_store_and_wait(void *dst_gmem, const void *src_smem, unsigned bytes) {
+// shared -> global, queued in the thread's current bulk group
+__device__ __forceinline__ void pg_bulk_store(void *dst_gmem, const void *src_smem, unsigned bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(pg_smem_addr(src_smem)), "r"(bytes) : "memory");
+}
+// returns once the engine has read the sources of the stores queued so far (the CTA may then exit / reuse them)
+__device__ __forceinline__ void pg_bulk_commit_and_wait() {
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
@@ -296,10 +299,11 @@ __device__ __forceinline__ void pg_bulk_store_and_wait(void *dst_gmem, const voi
 //   compose                warp w owns rows y = w (mod 4): gather (cells over background; a lane = 4 pixel
 //                          columns x 8 rows), then paint the entity blits in draw order, lanes sharing each blit
 //   pack + store           RGB32 -> RGB888 in place, one bulk copy of the 12 KiB frame to the observation buffer
+//                          (and, with a rollout, a second one to the env's rollout slot, in the same bulk group)
 // render_env_frame is that sequence for the env env_of() returns, on mbarrier phase `parity`. PASS: see
 // render_kernel. The env index and whether phase A's env ended its level are fetched where they are needed, so
-// that nothing stays live across the frame (the 8-CTA games have no register to spare).
-template <class G, int VIEW, int PASS, class EnvOf>
+// that nothing stays live across the frame (the 8-CTA games have no register to spare). ROLL: see render_kernel.
+template <class G, int VIEW, int PASS, bool ROLL, class EnvOf>
 __device__ __forceinline__ void render_env_frame(const KParams &p, typename FrameFor<G, VIEW>::type &f, EnvOf env_of, unsigned parity) {
     using Frame = typename FrameFor<G, VIEW>::type;
     const int tid = (int)threadIdx.x;
@@ -385,9 +389,16 @@ __device__ __forceinline__ void render_env_frame(const KParams &p, typename Fram
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of f.fb -> visible to the bulk copy
     __syncthreads();
     PG_RENDER_PHASE(6);
-    if (tid == 0)
-        pg_bulk_store_and_wait((PASS == 1 && p.level_end[env_of()] != 0 ? p.final_rgb : p.rgb) + (size_t)env_of() * (RES_W * RES_H * 3), f.fb,
-                               RES_W * RES_H * 3);
+    if (tid == 0) {
+        pg_bulk_store((PASS == 1 && p.level_end[env_of()] != 0 ? p.final_rgb : p.rgb) + (size_t)env_of() * (RES_W * RES_H * 3), f.fb,
+                      RES_W * RES_H * 3);
+        // the rollout's copy of the step's frame: a final frame is not one (phase B stores the env's next first frame)
+        if (ROLL && !(PASS == 1 && p.level_end[env_of()] != 0)) {
+            pg_bulk_store(p.roll.rgb + rollout_index(p, env_of()) * (RES_W * RES_H * 3), f.fb, RES_W * RES_H * 3);
+            rollout_store_scalars(p, env_of());
+        }
+        pg_bulk_commit_and_wait();
+    }
     PG_RENDER_PHASE(7);
 #undef PG_RENDER_PHASE
 }
@@ -407,14 +418,27 @@ __device__ __forceinline__ void consumer_repeat_frame(const KParams &p, int env)
     }
 }
 
+// A paused env's rollout slot: the frame it is paused on, rew = 0 and first = 0 (the step's outputs)
+__device__ __forceinline__ void rollout_repeat_frame(const KParams &p, int env) {
+    constexpr int kFrameVecs = RES_W * RES_H * 3 / 16;
+    const uint4 *src = reinterpret_cast<const uint4 *>(p.rgb) + (size_t)env * kFrameVecs;
+    uint4 *dst = reinterpret_cast<uint4 *>(p.roll.rgb) + rollout_index(p, env) * kFrameVecs;
+    for (int w = (int)threadIdx.x; w < kFrameVecs; w += kRenderThreads) dst[w] = src[w];
+    if (threadIdx.x == 0)
+        rollout_store_scalars(p, env);
+}
+
 // PASS 0: a plain step, one CTA per env of the launch. With final outputs (pgb200_get_final_outputs):
 // PASS 1 (phase A), the same grid, but the frame of an env whose level ended is its final frame: it goes to
 // final_rgb and skips the consumer epilogue, whose episode-start rule would read the previous step's first[env].
 // PASS 2 (phase B), a fixed grid whose CTAs loop over the envs phase A listed, after their reset: the mbarrier is
 // re-armed per env with alternating parity, and the bulk store's wait_group.read 0 has already released the frame.
 // PAUSE (PASS 0 and 1, a handle with a pause mask): the CTA of an env paused in this step renders nothing; its rgb
-// slot keeps the frame it is paused on, and the consumer ring gets that frame again (consumer_repeat_frame).
-template <class G, int VIEW, int PASS = 0, bool PAUSE = false>
+// slot keeps the frame it is paused on, and the consumer ring and the rollout get that frame again
+// (consumer_repeat_frame, rollout_repeat_frame).
+// ROLL: the handle has a rollout (pgb200_get_rollout), which every frame of the step is also stored to. A separate
+// instantiation, so that the render kernel of a handle without one keeps its registers and stack.
+template <class G, int VIEW, int PASS = 0, bool PAUSE = false, bool ROLL = false>
 __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlocks) render_kernel(KParams p) {
     static_assert(!(PAUSE && PASS == 2), "phase B's list never holds a paused env");
     using Frame = typename FrameFor<G, VIEW>::type;
@@ -423,6 +447,8 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
     if (PAUSE && p.paused[p.env_first + (int)blockIdx.x * p.env_step]) {
         if (p.consumer != nullptr && p.consumer_k > 1)
             consumer_repeat_frame(p, p.env_first + (int)blockIdx.x * p.env_step);
+        if (ROLL)
+            rollout_repeat_frame(p, p.env_first + (int)blockIdx.x * p.env_step);
         return;
     }
     if (threadIdx.x == 0)
@@ -438,12 +464,12 @@ __global__ void __launch_bounds__(kRenderThreads, RenderTune<G, VIEW>::kMinBlock
             if (threadIdx.x == 0)
                 list_env = p.reset_list[j];
             __syncthreads();
-            render_env_frame<G, VIEW, PASS>(p, f, [&] { return list_env; }, i & 1u);
+            render_env_frame<G, VIEW, PASS, ROLL>(p, f, [&] { return list_env; }, i & 1u);
             __syncthreads();
         }
         return;
     }
-    render_env_frame<G, VIEW, PASS>(p, f, [&] { return p.env_first + (int)blockIdx.x * p.env_step; }, 0);
+    render_env_frame<G, VIEW, PASS, ROLL>(p, f, [&] { return p.env_first + (int)blockIdx.x * p.env_step; }, 0);
 }
 
 #endif
@@ -462,8 +488,14 @@ __global__ void camera_kernel(KParams p) {
 }
 #endif
 
+// Host debug harness twin of the render kernel's rollout stores: env's rgb, rew and first of the step into its slot
+static inline void rollout_store_serial(const KParams &p, int env) {
+    memcpy(p.roll.rgb + rollout_index(p, env) * (RES_W * RES_H * 3), p.rgb + (size_t)env * (RES_W * RES_H * 3), RES_W * RES_H * 3);
+    rollout_store_scalars(p, env);
+}
+
 // the setup + render kernels' phases as plain loops (host debug harness; also documents the phase order). PASS: see
-// render_kernel; in pass 1 the frame of an env whose level ended goes to final_rgb.
+// render_kernel; in pass 1 the frame of an env whose level ended goes to final_rgb, and skips the rollout.
 template <class G, int VIEW, int PASS>
 void render_env_serial(const KParams &p, int env) {
     using Frame = typename FrameFor<G, VIEW>::type;
@@ -480,9 +512,12 @@ void render_env_serial(const KParams &p, int env) {
     static_cast<Shared &>(*f) = *reinterpret_cast<const Shared *>(p.frame_setup + (size_t)env * p.frame_setup_stride);
     env_stage_tiles_serial<Frame>(p, *f);
     for (int w = 0; w < 4; w++) env_render_compose<G, Frame>(p, *f, w, 4, 0, 1);  // the device's row ownership, one lane per owner
-    uint8_t *rgb = PASS == 1 && p.level_end[env] != 0 ? p.final_rgb : p.rgb;
+    const bool final_frame = PASS == 1 && p.level_end[env] != 0;
+    uint8_t *rgb = final_frame ? p.final_rgb : p.rgb;
     uint32_t *out = reinterpret_cast<uint32_t *>(rgb + (size_t)env * (RES_W * RES_H * 3));
     for (int g = 0; g < RES_W * RES_H / 4; g++) Raster<G, Frame>::pack_quad(f->fb + 4 * g, out + 3 * g);
+    if (p.roll.rgb != nullptr && !final_frame)
+        rollout_store_serial(p, env);
 }
 
 struct LaunchCtx {
@@ -504,7 +539,7 @@ struct LaunchCtx {
 #ifndef PG_HOSTSIM
 // Dynamic shared memory of one render CTA (frame, or the co-residency floor) with the kernel's
 // opt-in limit raised to it once.
-template <class G, int VIEW, int PASS = 0, bool PAUSE = false>
+template <class G, int VIEW, int PASS = 0, bool PAUSE = false, bool ROLL = false>
 int prepare_render_smem(const LaunchCtx &lc) {
     using Frame = typename FrameFor<G, VIEW>::type;
     const int bytes = (int)sizeof(Frame) > lc.render_smem_floor ? (int)sizeof(Frame) : lc.render_smem_floor;
@@ -514,7 +549,7 @@ int prepare_render_smem(const LaunchCtx &lc) {
     CUDA_CHECK(cudaGetDevice(&dev));
     int &have = attr_set[dev & 63];
     if (have < bytes) {
-        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS, PAUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        CUDA_CHECK(cudaFuncSetAttribute(render_kernel<G, VIEW, PASS, PAUSE, ROLL>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
         have = bytes;
     }
     return bytes;
@@ -613,13 +648,15 @@ void lookahead_phase(const KParams &p, const LaunchCtx &lc) {
 // frames: the setup kernel, then the render kernel of pass PASS, between kernel-timing events 1 to 3 (the runtime
 // gives a step with final outputs none). PASS 0 and 1 cover the launch's envs, and PAUSE leaves the paused ones'
 // frames as they are. PASS 2 covers the envs phase A listed: its grids are fixed (machine-filling) and read the
-// list's count on the device, so nothing waits for the host and the step stays capturable.
+// list's count on the device, so nothing waits for the host and the step stays capturable. A handle with a rollout
+// runs the render kernel's ROLL instantiation.
 template <class G, int VIEW, int PASS, bool PAUSE>
 void frames_phase(const KParams &p, const LaunchCtx &lc) {
     constexpr bool LIST = PASS == 2;
 #ifndef PG_HOSTSIM
     const int setup_smem = prepare_setup_smem<G, VIEW, LIST, PAUSE>();
-    const int render_smem = prepare_render_smem<G, VIEW, PASS, PAUSE>(lc);
+    const bool roll = p.roll.rgb != nullptr;
+    const int render_smem = roll ? prepare_render_smem<G, VIEW, PASS, PAUSE, true>(lc) : prepare_render_smem<G, VIEW, PASS, PAUSE, false>(lc);
     int setup_blocks = (p.env_count + kSetupThreads / 32 - 1) / (kSetupThreads / 32);
     int render_blocks = p.env_count;
     if (LIST) {
@@ -632,7 +669,10 @@ void frames_phase(const KParams &p, const LaunchCtx &lc) {
     setup_kernel<G, VIEW, LIST, PAUSE><<<setup_blocks, kSetupThreads, setup_smem, lc.stream>>>(p);
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[2], lc.stream));
-    render_kernel<G, VIEW, PASS, PAUSE><<<render_blocks, kRenderThreads, render_smem, lc.stream>>>(p);
+    if (roll)
+        render_kernel<G, VIEW, PASS, PAUSE, true><<<render_blocks, kRenderThreads, render_smem, lc.stream>>>(p);
+    else
+        render_kernel<G, VIEW, PASS, PAUSE, false><<<render_blocks, kRenderThreads, render_smem, lc.stream>>>(p);
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[3], lc.stream));
     CUDA_CHECK(cudaGetLastError());
@@ -646,6 +686,8 @@ void frames_phase(const KParams &p, const LaunchCtx &lc) {
         const int env = p.env_first + i * p.env_step;
         if (!(PAUSE && p.paused[env]))
             render_env_serial<G, VIEW, PASS>(p, env);
+        else if (p.roll.rgb != nullptr)
+            rollout_store_serial(p, env);
     }
 #endif
 }
@@ -722,9 +764,11 @@ void launch_env_kernel(const KParams &p, const LaunchCtx &lc) {
 }
 
 template <class G, int VIEW>
-void launch_observe_only(const KParams &p, const LaunchCtx &lc) {
-    if (p.env_count <= 0)
+void launch_observe_only(const KParams &step_params, const LaunchCtx &lc) {
+    if (step_params.env_count <= 0)
         return;
+    KParams p = step_params;  // an observation without a step leaves the rollout alone
+    p.roll.rgb = nullptr;
 #ifndef PG_HOSTSIM
     camera_kernel<G><<<p.env_count, 32, 0, lc.stream>>>(p);
     CUDA_CHECK(cudaGetLastError());

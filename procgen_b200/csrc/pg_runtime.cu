@@ -109,6 +109,9 @@ static inline void copy_to_dev_async(void *dst, const void *src, size_t bytes, S
 static inline void copy_from_dev_async(void *dst, const void *src, size_t bytes, Stream s) {
     CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
 }
+static inline void copy_dev_async(void *dst, const void *src, size_t bytes, Stream s) {
+    CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+}
 static inline void memset_async(void *dst, int value, size_t bytes, Stream s) { CUDA_CHECK(cudaMemsetAsync(dst, value, bytes, s)); }
 static inline void stream_sync(Stream s) { CUDA_CHECK(cudaStreamSynchronize(s)); }
 static inline void device_sync() { CUDA_CHECK(cudaDeviceSynchronize()); }
@@ -142,6 +145,7 @@ static inline void copy_to_dev(void *dst, const void *src, size_t bytes) { memcp
 static inline void copy_from_dev(void *dst, const void *src, size_t bytes) { memcpy(dst, src, bytes); }
 static inline void copy_to_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
 static inline void copy_from_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
+static inline void copy_dev_async(void *dst, const void *src, size_t bytes, Stream) { memcpy(dst, src, bytes); }
 static inline void memset_async(void *dst, int value, size_t bytes, Stream) { memset(dst, value, bytes); }
 static inline void stream_sync(Stream) {}
 static inline void device_sync() {}
@@ -270,9 +274,9 @@ __global__ void consumer_lut_kernel(uint16_t *lut, int bf16) {
     }
 }
 
-// The consumer ring position of the coming step, advanced on the device so that a step captured in a CUDA
-// graph moves it on at every replay (a kernel argument would be frozen at capture)
-__global__ void consumer_advance_kernel(int32_t *slot, int k) { *slot = (*slot + 1) % k; }
+// The ring position of the coming step (the consumer output's, the rollout's), advanced on the device so that a step
+// captured in a CUDA graph moves it on at every replay (a kernel argument would be frozen at capture)
+__global__ void ring_advance_kernel(int32_t *slot, int k) { *slot = (*slot + 1) % k; }
 #endif
 
 // ================================================================= VecEnv (VecGame, vecgame.h)
@@ -291,7 +295,8 @@ struct VecEnv {
     // next_level_seed by pgb200_get_next_level_seeds; final_rgb and level_end by pgb200_get_final_outputs;
     // pause (the caller's mask, d_pause) and paused (what the logic kernel recorded of it for the step's later
     // kernels) by pgb200_get_pause_mask; bank_level_end by the first pgb200_build_level_bank. reset_list, the
-    // pending-reset list of a two-phase step, by whichever of final outputs and the bank comes first.
+    // pending-reset list of a two-phase step, by whichever of final outputs and the bank comes first. The rollout
+    // (base.roll) by the first pgb200_get_rollout.
     uint8_t *d_pause = nullptr;
     // allocated by the first pgb200_build_level_bank: bank_capacity slots per game of the list, sized by the game
     // (banks[g], one allocation at base.bank.slots), the sorted seed list they share and its length on the device
@@ -456,7 +461,13 @@ struct VecEnv {
         // the consumer ring moves on once per step, behind the previous step and ahead of every render
         // kernel of this one (they all start after the fork below)
         if (!init && base.consumer) {
-            consumer_advance_kernel<<<1, 1, 0, stream>>>(d_consumer_slot, base.consumer_k);
+            ring_advance_kernel<<<1, 1, 0, stream>>>(d_consumer_slot, base.consumer_k);
+            CUDA_CHECK(cudaGetLastError());
+            launches++;
+        }
+        // so does the rollout's cursor
+        if (!init && base.roll.rgb) {
+            ring_advance_kernel<<<1, 1, 0, stream>>>(base.roll.cursor, base.roll.slots);
             CUDA_CHECK(cudaGetLastError());
             launches++;
         }
@@ -467,6 +478,11 @@ struct VecEnv {
                 if (priority_split)
                     CUDA_CHECK(cudaStreamWaitEvent(aux_hi[s], ev_fork, 0));
             }
+        }
+#else
+        if (!init && base.roll.rgb) {
+            *base.roll.cursor = (*base.roll.cursor + 1) % base.roll.slots;
+            launches++;
         }
 #endif
         if (!init && mirror[0])
@@ -1149,6 +1165,38 @@ int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
     v->opt_in_array(v->d_pause, 1, 0);
     v->base.pause = v->d_pause;
     *out = v->d_pause;
+    return 0;
+}
+
+int pgb200_get_rollout(libenv_env *handle, int slots, struct pgb200_rollout *out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    Rollout &r = v->base.roll;
+    const size_t frame = RES_W * RES_H * 3, N = (size_t)std::max(v->num_envs, 1);
+    if (slots < 2 || (r.rgb && slots != r.slots) || (size_t)slots > SIZE_MAX / (N * frame))
+        return -1;
+    if (!v->begin_opt_in(r.rgb != nullptr))
+        return -1;
+    if (!r.rgb) {
+        uint8_t *rgb = nullptr;
+        v->opt_in_array(rgb, (size_t)slots * frame, 0);
+        v->opt_in_array(r.rew, (size_t)slots, 0);
+        v->opt_in_array(r.first, (size_t)slots, 0);
+        r.cursor = v->alloc<int32_t>(1);  // slot 0
+        device_sync();                     // alloc's memset ran on the legacy stream
+        r.slots = slots;
+        r.num_envs = v->num_envs;
+        // slot 0 holds the outputs current now: those of the last step issued, or of the initial reset
+        copy_dev_async(rgb, v->base.rgb, (size_t)v->num_envs * frame, v->stream);
+        copy_dev_async(r.rew, v->base.rew, (size_t)v->num_envs * sizeof(float), v->stream);
+        copy_dev_async(r.first, v->base.first, (size_t)v->num_envs, v->stream);
+        v->sync();
+        r.rgb = rgb;  // last: a non-null rgb is what turns the rollout on
+    }
+    out->rgb = r.rgb;
+    out->rew = r.rew;
+    out->first = r.first;
+    out->cursor = r.cursor;
     return 0;
 }
 

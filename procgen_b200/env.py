@@ -138,6 +138,7 @@ class BaseProcgenEnv:
         self._next_level_seeds = None
         self._final_outputs = None
         self._pause_mask = None
+        self._rollout = None
         self._num_levels, self._start_level = num_levels, start_level
         self._consumer_slot = None
         self._graph_stepped = False   # act() has run inside a CUDA graph capture
@@ -274,9 +275,9 @@ class BaseProcgenEnv:
         Inside ``torch.cuda.graph`` (or any capture on the current stream) act() takes a CUDA tensor only and
         the step becomes part of the graph: the handle is rebound to the capture stream without a host wait,
         and every replay steps the envs again with whatever the action tensor then holds. Set up before the
-        capture what the step should use (next_level_seeds(), pause_mask(), enable_consumer_output(),
-        set_launch_shape()): a graph keeps the launch shape, the level choice, the pause mask and the consumer output
-        it was captured with."""
+        capture what the step should use (next_level_seeds(), pause_mask(), enable_consumer_output(), rollout(),
+        set_launch_shape()): a graph keeps the launch shape, the level choice, the pause mask, the consumer output and
+        the rollout it was captured with."""
         if self._capturing():
             if self._host_buffers:
                 raise RuntimeError("procgen_b200: act() cannot be captured in a CUDA graph with host_buffers=True; "
@@ -418,6 +419,40 @@ class BaseProcgenEnv:
                     raise RuntimeError("pgb200_get_pause_mask failed")
                 self._pause_mask = self._alias(ptr, (self.num,), "|u1")
         return self._pause_mask
+
+    def rollout(self, slots: int):
+        """{"rgb": uint8 [slots, num, 64, 64, 3], "rew": float32 [slots, num], "first": uint8 [slots, num], "cursor": int32
+        [1]}: CUDA tensors aliasing the library's rollout, a ring of `slots` copies of the step outputs. From the first
+        call on, every step (eager or replayed from a CUDA graph) moves cursor c on to (c + 1) % slots on the device and
+        stores its rgb, rew and first into slot c from the render kernel itself, byte for byte what observe() returns,
+        so a learner's rollout storage needs no copy after the step. The first call writes the current outputs into
+        slot 0 and sets cursor to 0. With final_outputs() a slot holds the next level's first frame (what rgb holds);
+        a paused env's slot holds the frame it is paused on, with rew = 0 and first = 0. get_state / set_state leave
+        the rollout alone. A rollout of T steps plus the observation to bootstrap from needs slots >= T + 1.
+
+        The memory (12 KiB per env and slot) is held until close(); there is no off switch, and `slots` is fixed by
+        the first call (ValueError for another value, or for slots < 2). A CUDA graph fills the rollout only if it
+        was requested before the capture: call this once first."""
+        slots = int(slots)
+        if self._rollout is not None:
+            if slots != self._rollout["rgb"].shape[0]:
+                raise ValueError(f"rollout(): this handle's rollout has {self._rollout['rgb'].shape[0]} slots")
+            return dict(self._rollout)
+        if slots < 2:
+            raise ValueError("rollout(): slots must be at least 2")
+        self._refuse_in_capture("rollout")
+        self._wait_for_replays()
+        torch = self._torch
+        out = L.Rollout()
+        with torch.cuda.device(self.device_index):
+            if self._lib.pgb200_get_rollout(self._h, slots, C.byref(out)) != 0:
+                raise RuntimeError("pgb200_get_rollout failed")
+            n = self.num
+            self._rollout = {"rgb": self._alias(out.rgb, (slots, n, 64, 64, 3), "|u1"),
+                             "rew": self._alias(out.rew, (slots, n), "<f4"),
+                             "first": self._alias(out.first, (slots, n), "|u1"),
+                             "cursor": self._alias(out.cursor, (1,), "<i4")}
+        return dict(self._rollout)
 
     def build_level_bank(self, seeds=None, capacity: int = 0) -> None:
         """Bank the levels of `seeds` (default: range(start_level, start_level + num_levels)) for every game of the
@@ -702,6 +737,7 @@ class BaseProcgenEnv:
             self._next_level_seeds = None
             self._final_outputs = None
             self._pause_mask = None
+            self._rollout = None
             self._lib.libenv_close(self._h)
             self._h = None
 

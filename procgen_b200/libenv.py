@@ -45,6 +45,10 @@ class FinalOutputs(C.Structure):
 LEVEL_END_GAME, LEVEL_END_TIMEOUT, LEVEL_END_CALLER = 1, 2, 3   # include/procgen_b200.h PGB200_LEVEL_END_*
 
 
+class Rollout(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("rew", C.c_void_p), ("first", C.c_void_p), ("cursor", C.c_void_p)]
+
+
 class DeviceBuffers(C.Structure):
     _fields_ = [("rgb", C.c_void_p), ("rew", C.c_void_p), ("first", C.c_void_p), ("prev_level_seed", C.c_void_p),
                 ("prev_level_complete", C.c_void_p), ("level_seed", C.c_void_p), ("action", C.c_void_p),
@@ -59,7 +63,7 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
            "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
            "pgb200_build_level_bank", "pgb200_level_bank_info", "pgb200_enable_level_lookahead",
-           "pgb200_level_lookahead_info"]
+           "pgb200_level_lookahead_info", "pgb200_get_rollout"]
 
 _lib = None
 
@@ -91,6 +95,8 @@ def bind(lib):
     lib.pgb200_enable_level_lookahead.restype = C.c_int
     lib.pgb200_level_lookahead_info.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     lib.pgb200_level_lookahead_info.restype = C.c_int
+    lib.pgb200_get_rollout.argtypes = [C.c_void_p, C.c_int, C.POINTER(Rollout)]
+    lib.pgb200_get_rollout.restype = C.c_int
     lib.pgb200_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     lib.pgb200_set_stream.restype = None
     lib.pgb200_get_errors.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
