@@ -70,7 +70,7 @@ struct KParams {
     uint8_t *final_rgb;         // [N][64][64][3]
     uint8_t *level_end;         // [N] why env's level ended in this step (PGB200_LEVEL_END_*), 0 = it did not
     int32_t *reset_list;        // this launch's own segment of an [N] list: the envs phase B resets
-    unsigned int *reset_count;  // entries in reset_list (device; beside the launch's ticket)
+    unsigned int *reset_count;  // entries in reset_list (device; a word of the launch's TicketSlot)
     // optional pause mask (pgb200_get_pause_mask); null = off. Only the logic kernel reads the caller's array: it
     // records each env's decision in `paused`, which the step's setup and render kernels read, so that every kernel
     // of one step agrees even if the caller rewrites the mask while the step runs
@@ -97,6 +97,34 @@ PG_HD void rollout_store_scalars(const KParams &p, int env) {
     const size_t i = rollout_index(p, env);
     p.roll.rew[i] = p.rew[env];
     p.roll.first[i] = p.first[env];
+}
+
+// env's rollout slot of this step gets its current rgb, rew and first, copied by `lane` of `nlanes` threads (the CTA
+// of a paused env; one thread in the host debug build, behind each rendered frame)
+PG_HD void rollout_copy_frame(const KParams &p, int env, int lane, int nlanes) {
+    constexpr int kFrameVecs = RES_W * RES_H * 3 / 16;
+    const BankVec *src = reinterpret_cast<const BankVec *>(p.rgb) + (size_t)env * kFrameVecs;
+    BankVec *dst = reinterpret_cast<BankVec *>(p.roll.rgb) + rollout_index(p, env) * kFrameVecs;
+    for (int w = lane; w < kFrameVecs; w += nlanes) dst[w] = src[w];
+    if (lane == 0)
+        rollout_store_scalars(p, env);
+}
+
+// Whether env's frame in render pass PASS is the final frame of its level: pass 1 (phase A of a step with final
+// outputs) of an env whose level ended. It goes to final_rgb, and neither the consumer output nor the rollout gets it.
+template <int PASS>
+PG_HD bool is_final_frame(const KParams &p, int env) { return PASS == 1 && p.level_end[env] != 0; }
+
+// If `when`, appends env to `list`, whose length is *count: on the device the calling warp's lane 0 does. The list and
+// its count are read only to append (the logic kernel's stack frame depends on it).
+PG_HD void list_append(bool when, int32_t *const &list, unsigned int *const &count, int env) {
+#if defined(__CUDA_ARCH__)
+    if (when && (threadIdx.x & 31u) == 0)
+        list[atomicAdd(count, 1u)] = env;
+#else
+    if (when)
+        list[(*count)++] = env;
+#endif
 }
 
 PG_HD Ctx make_ctx(const KParams &p, int env) {
@@ -148,6 +176,15 @@ PG_HD void env_init_logic(const KParams &p, int env) {
     h.initial_reset_complete = 1;
     Raster<G, Frame>::prepare_camera(c);
     write_step_outputs(p, env, h);
+}
+
+// Game::observe without a step (set_state, vecgame.cpp:454-456): the camera and the scalar outputs (game.cpp:160-164).
+// One thread.
+template <class G, class Frame>
+PG_HD void env_observe(const KParams &p, int env) {
+    Ctx c = make_ctx(p, env);
+    Raster<G, Frame>::prepare_camera(c);
+    write_step_outputs(p, env, *c.h);
 }
 
 #if defined(__CUDACC__)
@@ -250,6 +287,21 @@ PG_HD bool env_step_logic_final(const KParams &p, int env) {
     return do_reset;
 }
 
+// One env of the logic kernel: INIT the first reset, otherwise a step. PAUSE: unless the pause mask holds env still.
+// FINAL: phase A of a two-phase step, which appends env to p.reset_list when its level ends. LEVEL_CHOICE: see
+// env_step_logic (a two-phase step's resets take the caller's choice in phase B).
+template <class G, class Frame, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE>
+PG_HD void env_logic(const KParams &p, int env) {
+    static_assert(!(LEVEL_CHOICE && FINAL), "phase A never resets");
+    if (INIT)
+        env_init_logic<G, Frame>(p, env);
+    else if (PAUSE && env_pause_logic<FINAL>(p, env)) {
+    } else if (FINAL) {
+        list_append(env_step_logic_final<G, Frame>(p, env), p.reset_list, p.reset_count, env);
+    } else
+        env_step_logic<G, Frame, LEVEL_CHOICE>(p, env);
+}
+
 // Where a lookahead handle's reset takes its level from: the bank where it holds the seed (BANK), else the env's
 // lookahead slot where it holds the seed for options like the env's, else generation. Counts the choice in
 // p.look.served.
@@ -295,18 +347,18 @@ PG_HD void lookahead_predict(const KParams &p, int env, bool bank) {
     unsigned char *slot = lookahead_slot(p.look, env);
     if (slot_key(slot) == seed)
         return;
+    // lane 0 keys the slot once every lane has read the old key
 #if defined(__CUDA_ARCH__)
     __syncwarp();
-    if ((threadIdx.x & 31u) == 0) {
+    if ((threadIdx.x & 31u) == 0)
+#endif
+    {
         slot_key(slot) = seed;
         slot_usable(slot) = 0;
-        p.look.list[atomicAdd(p.look.count, 1u)] = env;
     }
+    list_append(true, p.look.list, p.look.count, env);
+#if defined(__CUDA_ARCH__)
     __syncwarp();
-#else
-    slot_key(slot) = seed;
-    slot_usable(slot) = 0;
-    p.look.list[(*p.look.count)++] = env;
 #endif
 }
 

@@ -345,10 +345,7 @@ struct VecEnv {
     int force_chunks = 0;            // measurement knobs (pgb200_set_launch_shape)
     bool serialize_launches = false;
     static constexpr int kMaxTickets = 64;   // launch slots in flight
-    // words per slot: the logic kernel's ticket; with final outputs also the pending-reset count and phase B's ticket;
-    // with level lookahead also its list's count and the lookahead kernel's ticket
-    static constexpr int kTicketWords = 8;
-    unsigned int *d_tickets = nullptr;
+    TicketSlot *d_tickets = nullptr;
     int max_logic_blocks = 1;        // logic blocks the device holds at once (device setup); the host build runs one env at a time
     int num_sms = 1;
     int render_smem_floor = 0;
@@ -444,6 +441,23 @@ struct VecEnv {
         return p;
     }
 
+    // The kernels the next step runs: the opt-ins `base` holds. This is the one place that reads their pointers as
+    // switches, and each entry point that turns one on assigns the pointer read here last, once the feature's arrays
+    // are complete, so that no step sees a half-built feature.
+    StepShape step_shape(bool init) const {
+        StepShape s;
+        s.init = init;
+        if (init)
+            return s;
+        s.level_choice = base.next_level_seed != nullptr;
+        s.pause = base.pause != nullptr;
+        s.final_outputs = base.level_end != nullptr;
+        s.bank = base.bank.slots != nullptr;
+        s.look = base.look.slot.slots != nullptr;
+        s.roll = base.roll.rgb != nullptr;
+        return s;
+    }
+
     // One step = for every (game, env chunk): logic kernel then render kernel. Chunks go round-robin
     // onto a few auxiliary streams forked from / joined to the handle's stream with events, so the
     // latency-bound logic kernel of one chunk overlaps the issue-bound render kernel of another on
@@ -457,6 +471,7 @@ struct VecEnv {
         // more than one (logic, render) pair in the step — env chunks of one game, or the games of a
         // joint list — are spread over the auxiliary streams so they overlap on the SMs
         const int nstreams = (chunks * G > 1 && !serialize_launches) ? kAuxStreams : 0;
+        const StepShape shape = step_shape(init);
 #ifndef PG_HOSTSIM
         // the consumer ring moves on once per step, behind the previous step and ahead of every render
         // kernel of this one (they all start after the fork below)
@@ -466,7 +481,7 @@ struct VecEnv {
             launches++;
         }
         // so does the rollout's cursor
-        if (!init && base.roll.rgb) {
+        if (shape.roll) {
             ring_advance_kernel<<<1, 1, 0, stream>>>(base.roll.cursor, base.roll.slots);
             CUDA_CHECK(cudaGetLastError());
             launches++;
@@ -480,7 +495,7 @@ struct VecEnv {
             }
         }
 #else
-        if (!init && base.roll.rgb) {
+        if (shape.roll) {
             *base.roll.cursor = (*base.roll.cursor + 1) % base.roll.slots;
             launches++;
         }
@@ -500,11 +515,11 @@ struct VecEnv {
                 p.env_first = g + lo * G;
                 p.env_step = G;
                 p.env_count = hi - lo;
-                if (base.reset_list)
+                if (shape.two_phase())
                     p.reset_list = base.reset_list + g * per_game + lo;  // the launch's own segment
                 LaunchCtx lc = lctx();
-                lc.ticket = d_tickets + (k % kMaxTickets) * kTicketWords;
-                if (base.look.slot.slots) {
+                lc.ticket = d_tickets + k % kMaxTickets;
+                if (shape.look) {
                     // launches that share a side stream run their lookahead kernels one after the other
                     const int side = k % kAuxStreams;
                     p.look.list = base.look.list + g * per_game + lo;
@@ -519,15 +534,12 @@ struct VecEnv {
                         lc.link = ev_link[k % nstreams];
                     }
                 }
-                if (timing && !base.level_end && tev_used + 4 <= tev_pool.size()) {
+                if (timing && !shape.final_outputs && tev_used + 4 <= tev_pool.size()) {
                     lc.tev = &tev_pool[tev_used];
                     tev_used += 4;
                     tev_envs.push_back(p.env_count);
                 }
-                if (init)
-                    games[g]->init[view[g]](p, lc);
-                else
-                    games[g]->step[view[g]](p, lc);
+                games[g]->step[view[g]](p, lc, shape);
 #ifndef PG_HOSTSIM
                 // libenv (host buffer) mode: start this chunk's observation DMA right behind its
                 // render kernel, on the same stream, so the copy of one chunk overlaps the kernels
@@ -554,7 +566,7 @@ struct VecEnv {
                 }
                 // the lookahead kernel joins the launch's stream behind everything above, which never waits for it;
                 // the step still ends with it, so that a captured step is self-contained
-                if (!init && lc.look_stream && hi > lo) {
+                if (shape.look && hi > lo) {
                     CUDA_CHECK(cudaEventRecord(look_join[k % kAuxStreams], lc.look_stream));
                     CUDA_CHECK(cudaStreamWaitEvent(lc.stream, look_join[k % kAuxStreams], 0));
                 }
@@ -843,7 +855,7 @@ libenv_env *libenv_make(int num_envs, const struct libenv_options options) {
             CUDA_CHECK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
     }
 #endif
-    v->d_tickets = v->alloc<unsigned int>(VecEnv::kMaxTickets * VecEnv::kTicketWords);
+    v->d_tickets = v->alloc<TicketSlot>(VecEnv::kMaxTickets);
 
     // ---- assets
     std::string pack_path = resource_root;
@@ -1150,7 +1162,7 @@ int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_outputs *ou
         return -1;
     v->opt_in_array(v->base.final_rgb, RES_W * RES_H * 3, 0);
     v->opt_in_array(v->base.reset_list, 1, 0);
-    v->opt_in_array(v->base.level_end, 1, 0);  // last: a non-null level_end is what selects the two-phase step
+    v->opt_in_array(v->base.level_end, 1, 0);  // last: VecEnv::step_shape reads a non-null level_end as final outputs on
     out->rgb = v->base.final_rgb;
     out->level_end = v->base.level_end;
     return 0;
@@ -1163,7 +1175,7 @@ int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
         return -1;
     v->opt_in_array(v->base.paused, 1, 0);
     v->opt_in_array(v->d_pause, 1, 0);
-    v->base.pause = v->d_pause;
+    v->base.pause = v->d_pause;  // last: VecEnv::step_shape reads a non-null pause as the mask on
     *out = v->d_pause;
     return 0;
 }
@@ -1191,7 +1203,7 @@ int pgb200_get_rollout(libenv_env *handle, int slots, struct pgb200_rollout *out
         copy_dev_async(r.rew, v->base.rew, (size_t)v->num_envs * sizeof(float), v->stream);
         copy_dev_async(r.first, v->base.first, (size_t)v->num_envs, v->stream);
         v->sync();
-        r.rgb = rgb;  // last: a non-null rgb is what turns the rollout on
+        r.rgb = rgb;  // last: VecEnv::step_shape reads a non-null rgb as the rollout on
     }
     out->rgb = r.rgb;
     out->rew = r.rew;
@@ -1237,7 +1249,7 @@ int pgb200_build_level_bank(libenv_env *handle, const int32_t *seeds, int count,
         unsigned char *slots = v->alloc<unsigned char>(total);
         for (LevelBank &b : v->banks) b.slots = slots + reinterpret_cast<size_t>(b.slots);
         v->bank_bytes = (int64_t)total + (int64_t)v->bank_capacity * (int64_t)sizeof(int32_t) + (int64_t)sizeof(int32_t);
-        // set last: a non-null slots pointer is what selects the bank's kernels
+        // set last: VecEnv::step_shape reads a non-null slots pointer as the bank on
         base.bank = v->banks[0];
         base.bank.slots = slots;
         device_sync();  // alloc's memsets ran on the legacy stream
@@ -1334,15 +1346,15 @@ int pgb200_enable_level_lookahead(libenv_env *handle) {
         p.env_step = G;
         p.env_count = per_game;
         p.look.list = base.look.list + g * per_game;
-        p.look.count = v->d_tickets;  // the list's count and the lookahead kernel's ticket
+        p.look.count = &v->d_tickets->look_count;  // the list's count and the lookahead kernel's ticket
         p.look.stage = stage.get();
         p.look.stage_warps = warps;
-        memset_async(v->d_tickets, 0, 2 * sizeof(unsigned int), v->stream);
+        memset_async(p.look.count, 0, 2 * sizeof(unsigned int), v->stream);
         LaunchCtx lc = v->lctx();
         v->games[g]->lookahead_fill(p, lc);
     }
     v->sync();  // then the staging is released
-    base.look.slot = v->looks[0].slot;  // last: a non-null slots pointer is what selects the lookahead kernels
+    base.look.slot = v->looks[0].slot;  // last: VecEnv::step_shape reads a non-null slots pointer as lookahead on
     return 0;
 }
 
@@ -1639,7 +1651,8 @@ int pgb200_kernel_timing_begin(libenv_env *handle, int max_launch_pairs) {
 #ifndef PG_HOSTSIM
     VecEnv *v = (VecEnv *)handle;
     v->set_device();
-    if (v->base.level_end || !v->try_sync())
+    // a step with final outputs renders in both of its phases, which one quadruple of events cannot time
+    if (v->step_shape(false).final_outputs || !v->try_sync())
         return -1;
     while ((int)v->tev_pool.size() < 4 * max_launch_pairs) {
         cudaEvent_t e;
