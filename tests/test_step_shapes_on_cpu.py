@@ -1,13 +1,12 @@
-"""Kernel launches per step for every combination of the six opt-ins, in the host debug build.
+"""Every combination of the six opt-ins of a step, in the host debug build: kernel launches and outputs.
 
-pgb200_kernel_launches counts what a step issues, and the host debug build counts the loops that stand for the kernels.
-Per (game, env chunk) launch, a plain step issues 3: logic, setup and render. A two-phase step without final outputs (a
-level bank or level lookahead) issues 4, with the finish kernel. A step with final outputs issues 6: it renders in both
-phases. Level lookahead adds its own kernel. The rollout adds one per step, the advance of its cursor. The level-seed
-overrides and the pause mask select other instantiations of the same kernels and add none."""
-import ctypes as C
-import itertools
-
+pgb200_kernel_launches counts what a step issues, and the host debug build counts the loops that stand for the kernels
+(step_shapes.expected_launches). test_outputs_per_step_shape also checks what the steps compute: step_shapes'
+lockstep driver runs every shape of one game, and the 8 semantic shapes (level choice x pause x final outputs) with the
+level bank, level lookahead and the rollout on for the 16-game list in 80 launches and the whole-world view, against
+the oracle (its records, tests/golden/step_shape_records.json.gz; the live oracle while recording them). Every output,
+final output, override entry, rollout slot and state blob is compared, and the launch count of every step. The GPU
+build runs the same driver on the same records in tests/test_gpu_step_shapes.py."""
 import pytest
 
 from final_obs_oracle import LibFinal
@@ -17,38 +16,24 @@ from level_seed_oracle import next_level_seeds
 from oracle.ref_env import RefVecEnv, default_pack, mt19937_actions
 from pause_oracle import pause_mask
 from rollout import get_rollout
+from step_shapes import (ALL_ON, MID_RUN_ORDERS, SHAPES, expected_launches, kernel_launches, mid_run_turn_on, run_case, semantic_shapes,
+                         shape_id, use_step_shape_records)
 
-OPT_INS = ("level_choice", "pause", "final", "bank", "look", "roll")
-SHAPES = [dict(zip(OPT_INS, bits)) for bits in itertools.product((False, True), repeat=len(OPT_INS))]
 KW = dict(distribution_mode="easy", num_levels=0, start_level=0, rand_seed=0)
 # (env name, envs, launch_shape): one game in one launch, and a two-game list cut into 3 chunks per game
 HANDLES = {"one_game": ("coinrun", 8, None), "two_games_3_chunks": ("coinrun,maze", 12, (3, False))}
 
 
-def _shape_id(shape):
-    return "+".join(k for k in OPT_INS if shape[k]) or "plain"
+@pytest.fixture(autouse=True, scope="module")
+def _step_shape_records():
+    use_step_shape_records()
 
 
-def expected_launches(shape, launches_per_step):
-    if shape["final"]:
-        per_launch = 6
-    elif shape["bank"] or shape["look"]:
-        per_launch = 4
-    else:
-        per_launch = 3
-    if shape["look"]:
-        per_launch += 1
-    return per_launch * launches_per_step + (1 if shape["roll"] else 0)
-
-
-@pytest.mark.parametrize("shape", SHAPES, ids=_shape_id)
+@pytest.mark.parametrize("shape", SHAPES, ids=shape_id)
 @pytest.mark.parametrize("handle", list(HANDLES))
 def test_launches_per_step(hostsim_lib, handle, shape):
     name, n, launch_shape = HANDLES[handle]
     env = RefVecEnv(n, name, lib_path=hostsim_lib, resource_root=default_pack(), launch_shape=launch_shape, **KW)
-    lib = env.lib
-    lib.pgb200_kernel_launches.argtypes = [C.c_void_p]
-    lib.pgb200_kernel_launches.restype = C.c_int64
     if shape["level_choice"]:
         next_level_seeds(env)
     if shape["pause"]:
@@ -65,7 +50,22 @@ def test_launches_per_step(hostsim_lib, handle, shape):
     games = len(name.split(","))
     launches_per_step = games * (launch_shape[0] if launch_shape else 1)
     for t, a in enumerate(mt19937_actions(3, n, 4)):
-        before = lib.pgb200_kernel_launches(C.c_void_p(env.h))
+        before = kernel_launches(env)
         env.act(a)
-        assert lib.pgb200_kernel_launches(C.c_void_p(env.h)) - before == expected_launches(shape, launches_per_step), f"step {t}"
+        assert kernel_launches(env) - before == expected_launches(shape, launches_per_step), f"step {t}"
     env.close()
+
+
+# all 64 shapes of one game; the 8 semantic shapes with bank, lookahead and rollout on for the other cases
+OUTPUT_RUNS = [("one_game", s) for s in SHAPES] + [(c, s) for c in ("sixteen_games", "whole_world") for s in semantic_shapes()]
+
+
+@pytest.mark.parametrize("case,shape", OUTPUT_RUNS, ids=[f"{c}-{shape_id(s)}" for c, s in OUTPUT_RUNS])
+def test_outputs_per_step_shape(hostsim_lib, case, shape):
+    run_case(case, hostsim_lib, shape)
+
+
+@pytest.mark.parametrize("order", list(MID_RUN_ORDERS))
+def test_outputs_with_opt_ins_turned_on_mid_run(hostsim_lib, order):
+    """One opt-in turned on every 4 steps, in three orders (the records test_gpu_step_shapes.py replays)"""
+    run_case("sixteen_games", hostsim_lib, ALL_ON, turn_on=mid_run_turn_on(order), label=f"mid_run_{order}")
