@@ -20,6 +20,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <memory>
 #include <random>
 #include <stdexcept>
@@ -1552,30 +1553,38 @@ int pgb200_debug_read_env(libenv_env *handle, int env, void *hdr_out, void *ents
 
 // ---- get_state / set_state (vecgame.cpp:437-457)
 
-static void fetch_env(VecEnv *v, int env, host::HostEnv &e) {
+// One env's records as (device address, host address, bytes), with the HostEnv sized to hold them.
+// get_state copies them down; set_state copies them down and, once the blob is read into them, back up.
+struct EnvRecord {
+    void *dev, *host;
+    size_t bytes;  // 0 for the scratch record of a game list without scratch words
+};
+using EnvRecords = std::array<EnvRecord, 6>;
+
+static EnvRecords env_records(VecEnv *v, int env, host::HostEnv &e) {
     const KParams &p = v->base;
     e.ent_cap = p.ent_stride - 1;
     e.ents.resize((size_t)p.ent_stride);
     e.grid.resize((size_t)p.grid_stride);
     e.scratch.resize((size_t)p.scratch_stride);
-    copy_from_dev(&e.h, p.hdr + env, sizeof(EnvHdr));
-    copy_from_dev(e.ents.data(), p.ents + (size_t)env * p.ent_stride, e.ents.size() * sizeof(Entity));
-    copy_from_dev(e.grid.data(), p.grid + (size_t)env * p.grid_stride, e.grid.size() * sizeof(int16_t));
-    copy_from_dev(&e.rng, p.rng + env, sizeof(MT19937));
-    copy_from_dev(&e.lvl_rng, p.lvl_rng + env, sizeof(MT19937));
-    if (!e.scratch.empty())
-        copy_from_dev(e.scratch.data(), p.scratch + (size_t)env * p.scratch_stride, e.scratch.size() * sizeof(int32_t));
+    return {{{p.hdr + env, &e.h, sizeof(EnvHdr)},
+             {p.ents + (size_t)env * p.ent_stride, e.ents.data(), e.ents.size() * sizeof(Entity)},
+             {p.grid + (size_t)env * p.grid_stride, e.grid.data(), e.grid.size() * sizeof(int16_t)},
+             {p.rng + env, &e.rng, sizeof(MT19937)},
+             {p.lvl_rng + env, &e.lvl_rng, sizeof(MT19937)},
+             {p.scratch + (size_t)env * p.scratch_stride, e.scratch.data(), e.scratch.size() * sizeof(int32_t)}}};
 }
 
-static void store_env(VecEnv *v, int env, const host::HostEnv &e) {
-    const KParams &p = v->base;
-    copy_to_dev(p.hdr + env, &e.h, sizeof(EnvHdr));
-    copy_to_dev(p.ents + (size_t)env * p.ent_stride, e.ents.data(), e.ents.size() * sizeof(Entity));
-    copy_to_dev(p.grid + (size_t)env * p.grid_stride, e.grid.data(), e.grid.size() * sizeof(int16_t));
-    copy_to_dev(p.rng + env, &e.rng, sizeof(MT19937));
-    copy_to_dev(p.lvl_rng + env, &e.lvl_rng, sizeof(MT19937));
-    if (!e.scratch.empty())
-        copy_to_dev(p.scratch + (size_t)env * p.scratch_stride, e.scratch.data(), e.scratch.size() * sizeof(int32_t));
+static void fetch_env(const EnvRecords &records) {
+    for (const EnvRecord &r : records)
+        if (r.bytes)
+            copy_from_dev(r.host, r.dev, r.bytes);
+}
+
+static void store_env(const EnvRecords &records) {
+    for (const EnvRecord &r : records)
+        if (r.bytes)
+            copy_to_dev(r.dev, r.host, r.bytes);
 }
 
 int get_state(libenv_env *handle, int env_idx, char *data, int length) {
@@ -1585,7 +1594,7 @@ int get_state(libenv_env *handle, int env_idx, char *data, int length) {
     if (!v->try_sync(true))  // wait_for_stepping_threads
         return -1;
     host::HostEnv e;
-    fetch_env(v, env_idx, e);
+    fetch_env(env_records(v, env_idx, e));
     const GameVTable *g = v->games[(size_t)env_idx % v->games.size()];
     try {
         host::WriteBuf b(data, (size_t)(length < 0 ? 0 : length));
@@ -1605,7 +1614,8 @@ void set_state(libenv_env *handle, int env_idx, char *data, int length) {
     v->ensure_initial_reset();
     v->sync();
     host::HostEnv e;
-    fetch_env(v, env_idx, e);  // capacities, game id and the fields the blob does not carry
+    const EnvRecords records = env_records(v, env_idx, e);
+    fetch_env(records);  // capacities, game id and the fields the blob does not carry
     const size_t gi = (size_t)env_idx % v->games.size();
     const GameVTable *g = v->games[gi];
     try {
@@ -1614,7 +1624,7 @@ void set_state(libenv_env *handle, int env_idx, char *data, int length) {
     } catch (const std::exception &ex) {
         pg_fatal("set_state: %s\n", ex.what());
     }
-    store_env(v, env_idx, e);
+    store_env(records);
     device_sync();  // the uploads ran on the legacy stream; the kernels below do not order against it
     // Game::observe(): re-render this env and rewrite its rew / first / info slots from the restored step_data
     KParams p = v->game_params((int)gi);
