@@ -133,7 +133,8 @@ LIBENV_API void libenv_close(libenv_env *handle);
  * state saved by the reference loads here and vice versa. get_state returns the number of bytes
  * written (a too small buffer is fatal, like the reference's fassert); set_state also re-renders
  * the env's observation and rewrites its rew / first / info slots from the restored state (Game::observe).
- * Both wait for the step in flight. */
+ * Both wait for the step in flight. They are the one-env case of pgb200_get_states / pgb200_set_states (Part 2);
+ * a malformed blob is fatal with `fatal: set_state: <check> (env <index>)`. */
 LIBENV_API int get_state(libenv_env *handle, int env_idx, char *data, int length);
 LIBENV_API void set_state(libenv_env *handle, int env_idx, char *data, int length);
 
@@ -311,6 +312,24 @@ struct pgb200_rollout {
     int32_t *cursor;  /* [1]: the slot the latest step (or the first call) wrote */
 };
 LIBENV_API int pgb200_get_rollout(libenv_env *handle, int slots, struct pgb200_rollout *out);
+
+/* States of chosen envs in one call: get_state / set_state for the list envs[0, n) (host memory; the handle's own
+ * indices), with the blobs in the same wire format, and no host round trip per env. On the device, each listed env's
+ * header, generators, live entities, live grid cells and persistent scratch words are gathered into (or scattered
+ * from) staging that a call grows up to 256 MiB, device and pinned each, and holds until libenv_close; the host
+ * writes and reads the blobs from those records.
+ * pgb200_get_states: the blob of envs[i] is (*data)[(*offsets)[i], (*offsets)[i + 1]). Both arrays are owned by
+ * the handle and stay valid until the next pgb200_get_states on it, or libenv_close. Duplicate entries are allowed.
+ * Waits for the step in flight, as get_state does, and performs the initial reset if it has not happened yet.
+ * Returns 0, or -1 (nothing changed) for n < 0, an env out of range, or while the handle's stream is capturing.
+ * pgb200_set_states: for each listed env, what set_state does: the blob data[offsets[i], offsets[i + 1]) is loaded,
+ * the env's frame re-rendered and its rew, first and info slots rewritten from the restored state (with the consumer
+ * output on, its current ring slot too). Envs not listed, the rollout, the pause mask, next_level_seed, final outputs,
+ * the bank and lookahead slots are untouched. Every blob is read before any env changes; a malformed one is fatal,
+ * `fatal: set_state: <check> (env <index>)`. Returns 0 once done, or -1 (nothing changed) for n < 0, an env out of
+ * range, an env listed twice, or while the handle's stream is capturing. */
+LIBENV_API int pgb200_get_states(libenv_env *handle, const int32_t *envs, int n, const char **data, const int64_t **offsets);
+LIBENV_API int pgb200_set_states(libenv_env *handle, const int32_t *envs, int n, const char *data, const int64_t *offsets);
 
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies

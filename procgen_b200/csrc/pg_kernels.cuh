@@ -187,6 +187,63 @@ PG_HD void env_observe(const KParams &p, int env) {
     write_step_outputs(p, env, *c.h);
 }
 
+// ---- state transfers (get_state / set_state and their batched forms). The device moves, per listed env, exactly the
+// part of its records that the state blob is written from or read into (pg_state_io.h io_env): the header, both
+// generators, the live entities, the main_width x main_height grid cells and the game's persistent scratch words. They
+// travel as one packed record per env, each part 16-byte aligned:
+//   EnvHdr | rand_gen | level_seed_rand_gen | Entity[n_ents] | int16 grid[cells] | int32 scratch[scratch_words]
+// The host serializes from and deserializes into those records; everything else of the env stays where it is.
+struct StateSlot {
+    int32_t env;
+    int32_t n_ents;         // entities [0, n_ents)
+    int32_t cells;          // grid cells [0, cells)
+    int32_t scratch_first;  // scratch words [scratch_first, scratch_first + scratch_words)
+    int32_t scratch_words;
+    int32_t pad;
+    int64_t offset;         // of the packed record, in bytes from the start of its chunk's records
+};
+
+PG_HD size_t state_ents_off() { return sizeof(EnvHdr) + 2 * sizeof(MT19937); }
+PG_HD size_t state_grid_off(const StateSlot &s) { return state_ents_off() + (size_t)s.n_ents * sizeof(Entity); }
+PG_HD size_t state_scratch_off(const StateSlot &s) { return state_grid_off(s) + (((size_t)s.cells * sizeof(int16_t) + 15) & ~(size_t)15); }
+PG_HD size_t state_record_bytes(const StateSlot &s) {
+    return state_scratch_off(s) + (((size_t)s.scratch_words * sizeof(int32_t) + 15) & ~(size_t)15);
+}
+
+// s.env's records -> the packed record `rec` (STORE false), or `rec` -> the env's records (STORE true). One warp (one
+// thread in the host debug build).
+template <bool STORE>
+PG_HD void state_move(const KParams &p, const StateSlot &s, unsigned char *rec) {
+    static_assert(sizeof(EnvHdr) % 16 == 0 && sizeof(MT19937) % 16 == 0, "16-byte parts");
+    const int env = s.env;
+    auto vecs = [](void *env_part, unsigned char *rec_part, size_t bytes) {
+        if (STORE)
+            bank_copy_vecs(env_part, rec_part, (int)bytes);
+        else
+            bank_copy_vecs(rec_part, env_part, (int)bytes);
+    };
+    vecs(p.hdr + env, rec, sizeof(EnvHdr));
+    vecs(p.rng + env, rec + sizeof(EnvHdr), sizeof(MT19937));
+    vecs(p.lvl_rng + env, rec + sizeof(EnvHdr) + sizeof(MT19937), sizeof(MT19937));
+    vecs(p.ents + (size_t)env * p.ent_stride, rec + state_ents_off(), (size_t)s.n_ents * sizeof(Entity));
+    int16_t *grid = p.grid + (size_t)env * p.grid_stride;
+    int16_t *rec_grid = reinterpret_cast<int16_t *>(rec + state_grid_off(s));
+    pg_warp_for(s.cells, [=](int k) {
+        if (STORE)
+            grid[k] = rec_grid[k];
+        else
+            rec_grid[k] = grid[k];
+    });
+    int32_t *scratch = p.scratch + (size_t)env * p.scratch_stride + s.scratch_first;
+    int32_t *rec_scratch = reinterpret_cast<int32_t *>(rec + state_scratch_off(s));
+    pg_warp_for(s.scratch_words, [=](int k) {
+        if (STORE)
+            scratch[k] = rec_scratch[k];
+        else
+            rec_scratch[k] = scratch[k];
+    });
+}
+
 #if defined(__CUDACC__)
 // Warm the env's working set. A step's logic is one long dependent chain; touched cold, every
 // entity record / header line / grid row costs a serial DRAM round trip. Here the 32 lanes issue

@@ -465,6 +465,14 @@ __global__ void camera_kernel(KParams p) {
     if (threadIdx.x == 0 && blockIdx.x < (unsigned)p.env_count)
         env_observe<G, Frame>(p, p.env_first + (int)blockIdx.x * p.env_step);
 }
+
+// The same camera for the envs p.reset_list holds (set_state of a list of envs): block j takes entry j
+template <class G>
+__global__ void camera_list_kernel(KParams p) {
+    using Frame = typename FrameFor<G>::type;
+    if (threadIdx.x == 0 && blockIdx.x < *p.reset_count)
+        env_observe<G, Frame>(p, p.reset_list[blockIdx.x]);
+}
 #endif
 
 // the setup + render kernels' phases as plain loops (host debug harness; also documents the phase order). PASS and
@@ -753,6 +761,24 @@ void launch_observe_only(const KParams &p, const LaunchCtx &lc) {
     frames_phase<G, VIEW, 0>(p, lc, StepShape{});
 }
 
+// launch_observe_only for the p.env_count envs p.reset_list holds (*p.reset_count on the device), distinct envs of the
+// launch's game: the list camera, then the frames of phase B of a step without rollout. Phase B's render pass differs
+// from pass 0 only in taking its envs from the list, so the listed envs get what launch_observe_only gives them (rgb,
+// rew, first, the infos and the consumer ring's current slot) and the rollout is left alone. Counted as launch_observe_only.
+template <class G, int VIEW>
+void launch_observe_list(const KParams &p, const LaunchCtx &lc) {
+    if (p.env_count <= 0)
+        return;
+#ifndef PG_HOSTSIM
+    camera_list_kernel<G><<<p.env_count, 32, 0, lc.stream>>>(p);
+    CUDA_CHECK(cudaGetLastError());
+#else
+    using Frame = typename FrameFor<G>::type;
+    for (unsigned int j = 0; j < *p.reset_count; j++) env_observe<G, Frame>(p, p.reset_list[j]);
+#endif
+    frames_phase<G, VIEW, 2>(p, lc, StepShape{});
+}
+
 // Generates p.bank's levels [0, count) of the launch's game: `warps` warps, each with bank_stage_bytes(p) of `stage`.
 // Counted as a launch in the device build only.
 template <class G>
@@ -806,9 +832,10 @@ struct GameVTable {
     int render_ctas_per_sm[2];  // residency the render kernel is compiled for
     void (*step[2])(const KParams &, const LaunchCtx &, const StepShape &);  // a step or the initial reset (launch_step)
     void (*observe_only[2])(const KParams &, const LaunchCtx &);
+    void (*observe_list[2])(const KParams &, const LaunchCtx &);
     void (*bank_build)(const KParams &, const LaunchCtx &, unsigned char *, int, int);
     void (*lookahead_fill)(const KParams &, const LaunchCtx &);
-    int persist_scratch_words;  // G::PERSIST_SCRATCH_WORDS
+    int persist_scratch_first, persist_scratch_words;  // G::PERSIST_SCRATCH_FIRST / _WORDS
 };
 
 template <class G, int VIEW>
@@ -824,6 +851,7 @@ void fill_view(GameVTable &vt, int slot) {
 #endif
     vt.step[slot] = &launch_step<G, VIEW>;
     vt.observe_only[slot] = &launch_observe_only<G, VIEW>;
+    vt.observe_list[slot] = &launch_observe_list<G, VIEW>;
 }
 
 template <class G>
@@ -834,6 +862,7 @@ GameVTable make_vtable(int id) {
     vt.ent_cap = G::ENT_CAP;
     vt.grid_cap = G::GRID_CAP;
     vt.scratch_words = G::SCRATCH_WORDS;
+    vt.persist_scratch_first = G::PERSIST_SCRATCH_FIRST;
     vt.persist_scratch_words = G::PERSIST_SCRATCH_WORDS;
     vt.bank_build = &launch_bank_build<G>;
     vt.lookahead_fill = &launch_lookahead_fill<G>;

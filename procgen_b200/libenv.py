@@ -63,7 +63,7 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
            "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
            "pgb200_build_level_bank", "pgb200_level_bank_info", "pgb200_enable_level_lookahead",
-           "pgb200_level_lookahead_info", "pgb200_get_rollout"]
+           "pgb200_level_lookahead_info", "pgb200_get_rollout", "pgb200_get_states", "pgb200_set_states"]
 
 _lib = None
 
@@ -123,6 +123,11 @@ def bind(lib):
     lib.get_state.restype = C.c_int
     lib.set_state.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
     lib.set_state.restype = None
+    lib.pgb200_get_states.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_void_p),
+                                      C.POINTER(C.POINTER(C.c_int64))]
+    lib.pgb200_get_states.restype = C.c_int
+    lib.pgb200_set_states.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_char_p, C.POINTER(C.c_int64)]
+    lib.pgb200_set_states.restype = C.c_int
     lib.pgb200_set_launch_shape.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.pgb200_set_launch_shape.restype = None
     lib.pgb200_kernel_timing_begin.argtypes = [C.c_void_p, C.c_int]
