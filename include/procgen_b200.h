@@ -331,6 +331,48 @@ LIBENV_API int pgb200_get_rollout(libenv_env *handle, int slots, struct pgb200_r
 LIBENV_API int pgb200_get_states(libenv_env *handle, const int32_t *envs, int n, const char **data, const int64_t **offsets);
 LIBENV_API int pgb200_set_states(libenv_env *handle, const int32_t *envs, int n, const char *data, const int64_t *offsets);
 
+/* Snapshot slots: env states saved into and loaded from a store of `slots` slots on the device, without the host and
+ * without the wire format, so that an RL loop can clone envs, branch a state into several envs, or return envs to
+ * archived states inside its own device work (CUDA graphs included). Three int32 arrays of device memory (host memory
+ * in the CPU debug build) control it, every entry -1 at first:
+ *   save_from  [slots]     the caller's: at the next apply, slot s takes the state of env save_from[s]
+ *   load_from  [num_envs]  the caller's: at the next apply, env e takes the state slot load_from[e] holds
+ *   source     [slots]     read only: the env whose state slot s holds, -1 while it is empty
+ * pgb200_apply_snapshots enqueues on the handle's stream, in this order:
+ *   1. saves: every slot s with save_from[s] in [0, num_envs) takes that env's state; source[s] = that env and
+ *      save_from[s] = -1;
+ *   2. loads: every env e whose load_from[e] = s is a slot in [0, slots) that holds a state of e's own game
+ *      (source[s] % G == e % G, G the games of the list) takes that state; load_from[e] = -1;
+ *   3. every env loaded is observed as set_state observes it: its rgb, rew, first and info slots (and with the consumer
+ *      output on, its current ring slot) are rewritten from the loaded state.
+ * An entry that is not applied (an env or slot out of range, an empty slot, a slot of another game) keeps its value and
+ * changes nothing. Saves run before loads, so one call can clone (save_from[s] = a, load_from[b] = s), and an env may
+ * be saved and loaded in one call. After a load, env e's header (error bits, counters and high-water marks included),
+ * both generators, live entities, live grid cells and persistent scratch words are a byte-for-byte copy of the source
+ * env's at save time; so get_state(e) returns the blob get_state(source) returned then, and e steps on as the source
+ * would have. Envs not loaded, the rollout, final outputs, the pause mask (a paused env loaded stays paused),
+ * next_level_seed (pending overrides survive), the bank and lookahead slots (a slot keyed for the old state misses
+ * once) are left alone; the peer mirror is refreshed by the next step. A slot holds the handle's own layout: it is not
+ * portable across handles, builds or processes and is freed by libenv_close; get_state is the portable form.
+ * pgb200_get_snapshots: *out = the arrays and the device bytes the store holds (slots of about 80 KB each for coinrun:
+ * every slot is sized for the largest live state of the list). The first call performs the initial reset if it has not
+ * happened yet, allocates the store, waits and returns 0; a later call with the same `slots` returns the same pointers.
+ * Returns -1 (nothing changed) for slots < 1, a byte size that overflows, a failed allocation, a later call with other
+ * `slots`, or a first call while the handle's stream is capturing.
+ * pgb200_apply_snapshots: returns 0 once enqueued, or -1 on a handle without a store. It never waits for the host and
+ * may be captured in a CUDA graph; each replay reads the arrays as they are then. Ordering as for next_level_seed:
+ * write the arrays on the handle's stream before the call (with host buffers, the writes must be complete before the
+ * call). pgb200_kernel_launches counts 2 + 2 * G per call: the save and load kernels, and each game's two frame
+ * kernels (as set_state's observe, its camera kernel is not counted). */
+struct pgb200_snapshots {
+    int32_t *save_from;     /* [slots] */
+    int32_t *load_from;     /* [num_envs] */
+    const int32_t *source;  /* [slots] */
+    int64_t bytes;          /* device memory the store holds */
+};
+LIBENV_API int pgb200_get_snapshots(libenv_env *handle, int slots, struct pgb200_snapshots *out);
+LIBENV_API int pgb200_apply_snapshots(libenv_env *handle);
+
 /* Re-home all subsequent work of this handle onto the caller's stream (a cudaStream_t, e.g. the
  * framework's current stream) so launches are ordered with the caller's own kernels and copies
  * without events. The handle's previous work is drained first. The value is used literally: NULL is
@@ -352,11 +394,11 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * before the capture; likewise the pause mask and pgb200_get_pause_mask), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
  * any of these afterwards leaves the graph as it was; capture again. Replays of one handle's graphs must be
  * ordered with each other and with its eager work (one stream, or events). pgb200_kernel_launches counts
- * launches issued, a captured step once, not its replays.
+ * launches issued, a captured step once, not its replays. pgb200_apply_snapshots may be captured the same way.
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
  * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank,
- * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, the first pgb200_get_rollout, pgb200_get_device_buffers
+ * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, the first pgb200_get_rollout, the first pgb200_get_snapshots, pgb200_get_device_buffers
  * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,
  * pgb200_set_launch_shape, pgb200_kernel_timing_begin / _end, pgb200_sync and the libenv_* calls. A step

@@ -244,6 +244,79 @@ PG_HD void state_move(const KParams &p, const StateSlot &s, unsigned char *rec) 
     });
 }
 
+// ---- snapshot slots (pgb200_get_snapshots / pgb200_apply_snapshots): packed records kept in a handle-owned store on
+// the device. Every slot has the same size, set by the handle's strides, and holds
+//   StateSlot (the record's sizes, as state_slot() makes them) | Entity ghost | the packed record
+// The ghost is entity slot ent_cap, where erase_if_needed moves an agent it erases (agent_idx == ent_cap). Nothing in
+// a step resets an env on that alone (step_play's done tests the agent against the world's bounds, not its erasure),
+// so the code does not rule out such a state between steps, and a snapshot carries the ghost with the record. get_state
+// refuses that state instead, since the wire format has no place for the ghost.
+struct SnapshotStore {
+    unsigned char *slots;     // [count][slot_bytes]; null: the handle has no store
+    int64_t slot_bytes;
+    int32_t count;            // slots
+    int32_t num_envs;
+    int32_t games;            // env e plays game e % games of the list
+    int32_t pad;
+    int32_t *save_from;       // [count] the caller's: env whose state slot s takes at the next apply, -1 = none
+    int32_t *load_from;       // [num_envs] the caller's: slot env e takes at the next apply, -1 = none
+    int32_t *source;          // [count] env whose state slot s holds, -1 = empty
+    const int32_t *persist;   // [games][2] each game's PERSIST_SCRATCH_FIRST and _WORDS
+    int32_t *list;            // [num_envs] the envs an apply loaded: game g's at [g, g + 1) * num_envs / games
+    unsigned int *counts;     // [games] entries in each game's segment of `list`
+};
+
+constexpr size_t kSnapshotGhostOff = sizeof(StateSlot);
+constexpr size_t kSnapshotRecordOff = kSnapshotGhostOff + sizeof(Entity);
+static_assert(sizeof(StateSlot) % 16 == 0, "16-byte slot parts");
+
+// Slot s takes the current state of env save_from[s], if that is in [0, num_envs): the packed record of the env's live
+// part and its ghost entity; then source[s] = env and save_from[s] = -1. One warp (one thread in the host debug build).
+PG_HD void snapshot_save(const KParams &p, const SnapshotStore &st, int s) {
+    const int env = st.save_from[s];
+    if (env < 0 || env >= st.num_envs)
+        return;
+    const EnvHdr &h = p.hdr[env];
+    const int64_t cells = (int64_t)h.main_width * h.main_height;
+    StateSlot d{};
+    d.env = env;
+    d.n_ents = h.n_ents < 0 ? 0 : (h.n_ents < p.ent_stride - 1 ? h.n_ents : p.ent_stride - 1);
+    d.cells = cells < 0 ? 0 : (int)(cells < p.grid_stride ? cells : p.grid_stride);
+    d.scratch_first = st.persist[2 * (env % st.games)];
+    d.scratch_words = st.persist[2 * (env % st.games) + 1];
+    unsigned char *slot = st.slots + (size_t)s * (size_t)st.slot_bytes;
+    state_move<false>(p, d, slot + kSnapshotRecordOff);
+    bank_copy_vecs(slot + kSnapshotGhostOff, p.ents + (size_t)env * p.ent_stride + (p.ent_stride - 1), (int)sizeof(Entity));
+    // every lane has read save_from[s] before the warp_for barriers above
+    pg_warp_for(1, [=](int) {
+        *reinterpret_cast<StateSlot *>(slot) = d;
+        st.source[s] = env;
+        st.save_from[s] = -1;
+    });
+}
+
+// Env takes the state slot load_from[env] holds, if the slot is in [0, count), holds a state, and of the env's own game;
+// then it is appended to its game's segment of `list` and load_from[env] = -1. An entry refused stays as it is. One
+// warp (one thread in the host debug build).
+PG_HD void snapshot_load(const KParams &p, const SnapshotStore &st, int env) {
+    const int s = st.load_from[env];
+    if (s < 0 || s >= st.count)
+        return;
+    const int src = st.source[s];
+    if (src < 0 || src % st.games != env % st.games)
+        return;
+    unsigned char *slot = st.slots + (size_t)s * (size_t)st.slot_bytes;
+    StateSlot d = *reinterpret_cast<const StateSlot *>(slot);
+    d.env = env;
+    state_move<true>(p, d, slot + kSnapshotRecordOff);
+    bank_copy_vecs(p.ents + (size_t)env * p.ent_stride + (p.ent_stride - 1), slot + kSnapshotGhostOff, (int)sizeof(Entity));
+    const int g = env % st.games;
+    int32_t *const seg = st.list + (size_t)g * (size_t)(st.num_envs / st.games);
+    unsigned int *const count = st.counts + g;
+    list_append(true, seg, count, env);
+    pg_warp_for(1, [=](int) { st.load_from[env] = -1; });
+}
+
 #if defined(__CUDACC__)
 // Warm the env's working set. A step's logic is one long dependent chain; touched cold, every
 // entity record / header line / grid row costs a serial DRAM round trip. Here the 32 lanes issue

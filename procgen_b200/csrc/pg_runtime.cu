@@ -88,6 +88,15 @@ static inline void *dev_malloc(size_t bytes) {
     return ptr;
 }
 static inline void dev_free(void *ptr) { cudaFree(ptr); }
+// device memory, or null when the device cannot provide it
+static inline void *dev_try_malloc(size_t bytes) {
+    void *ptr = nullptr;
+    if (cudaMalloc(&ptr, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return nullptr;
+    }
+    return ptr;
+}
 static inline void *pinned_alloc(size_t bytes) {
     void *ptr = nullptr;
     CUDA_CHECK(cudaHostAlloc(&ptr, bytes, cudaHostAllocDefault));
@@ -136,6 +145,7 @@ static constexpr int kDeviceBuild = 0;
 static inline void set_current_device(int) {}
 static inline void *dev_malloc(size_t bytes) { return calloc(bytes, 1); }
 static inline void dev_free(void *ptr) { free(ptr); }
+static inline void *dev_try_malloc(size_t bytes) { return calloc(bytes, 1); }
 static inline void *pinned_alloc(size_t bytes) { return malloc(bytes); }
 static inline void pinned_free(void *ptr) { free(ptr); }
 static inline void host_unregister(void *) {}
@@ -296,6 +306,19 @@ __global__ void __launch_bounds__(128) state_records_kernel(KParams p, const Sta
     if (i < count)
         state_move<STORE>(p, slots[i], recs + slots[i].offset);
 }
+
+// Snapshot slots (pgb200_apply_snapshots): the saves, one warp per slot, then the loads, one warp per env
+__global__ void __launch_bounds__(128) snapshot_save_kernel(KParams p, SnapshotStore st) {
+    const int s = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (s < st.count)
+        snapshot_save(p, st, s);
+}
+
+__global__ void __launch_bounds__(128) snapshot_load_kernel(KParams p, SnapshotStore st) {
+    const int env = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (env < st.num_envs)
+        snapshot_load(p, st, env);
+}
 #endif
 
 // ================================================================= VecEnv (VecGame, vecgame.h)
@@ -399,6 +422,9 @@ struct VecEnv {
     size_t state_stage_bytes = 0;
     std::vector<char> state_blobs;
     std::vector<int64_t> state_offsets;
+    // snapshot slots: allocated by the first pgb200_get_snapshots (snaps.slots null until then), snap_bytes in all
+    SnapshotStore snaps{};
+    int64_t snap_bytes = 0;
 
     VecEnv() = default;
     VecEnv(const VecEnv &) = delete;
@@ -1778,6 +1804,22 @@ int serialize_state(const VecEnv *v, int env, const host::HostEnv &e, char *data
     return (int)b.offset;
 }
 
+// Game::observe of the envs listed per game, on the handle's stream: game g's are the first *(counts + g) of
+// lists + first[g], a count read on the device and at most bound[g], which sizes the list camera's grid. One
+// launch_observe_list per game with bound[g] > 0.
+void observe_lists(VecEnv *v, int32_t *lists, unsigned int *counts, const std::vector<size_t> &first, const std::vector<uint32_t> &bound) {
+    for (size_t g = 0; g < v->games.size(); g++) {
+        if (bound[g] == 0)
+            continue;
+        KParams p = v->game_params((int)g);
+        p.reset_list = lists + first[g];
+        p.reset_count = counts + g;
+        p.env_count = (int)bound[g];
+        LaunchCtx lc = v->lctx();
+        v->games[g]->observe_list[v->view[g]](p, lc);
+    }
+}
+
 // Game::observe of envs[0, n) (distinct, the handle's stream idle): one launch_observe_list per game with listed envs
 void observe_states(VecEnv *v, const int32_t *envs, int n) {
     const size_t G = v->games.size();
@@ -1793,16 +1835,8 @@ void observe_states(VecEnv *v, const int32_t *envs, int n) {
     for (int i = 0; i < n; i++) h_lists[next[(size_t)envs[i] % G]++] = envs[i];
     memcpy(v->h_state_stage, counts.data(), G * sizeof(uint32_t));
     copy_to_dev_async(v->d_state_stage, v->h_state_stage, lists_off + (size_t)n * sizeof(int32_t), v->stream);
-    for (size_t g = 0; g < G; g++) {
-        if (counts[g] == 0)
-            continue;
-        KParams p = v->game_params((int)g);
-        p.reset_list = reinterpret_cast<int32_t *>(v->d_state_stage + lists_off) + first[g];
-        p.reset_count = reinterpret_cast<unsigned int *>(v->d_state_stage) + g;
-        p.env_count = (int)counts[g];
-        LaunchCtx lc = v->lctx();
-        v->games[g]->observe_list[v->view[g]](p, lc);
-    }
+    observe_lists(v, reinterpret_cast<int32_t *>(v->d_state_stage + lists_off), reinterpret_cast<unsigned int *>(v->d_state_stage),
+                  first, counts);
     v->sync();
     v->rgb_copy_enqueued = false;  // a DMA started behind the last step predates these frames: observe copies again
 }
@@ -1927,6 +1961,86 @@ void set_state(libenv_env *handle, int env_idx, char *data, int length) {
     v->sync();
     const int64_t offsets[2] = {0, length < 0 ? 0 : length};
     load_states(v, &env_idx, 1, data, offsets);
+}
+
+// ---- snapshot slots (SnapshotStore, pg_kernels.cuh). One allocation holds the caller's arrays, the load list, the
+// per-game table and the slots, each part 16-byte aligned.
+int pgb200_get_snapshots(libenv_env *handle, int slots, struct pgb200_snapshots *out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    SnapshotStore &st = v->snaps;
+    if (!out || slots < 1 || (st.slots && slots != st.count))
+        return -1;
+    if (!st.slots) {
+        const KParams &p = v->base;
+        const size_t G = v->games.size(), N = (size_t)v->num_envs, S = (size_t)slots;
+        StateSlot widest{};
+        widest.n_ents = p.ent_stride - 1;
+        widest.cells = p.grid_stride;
+        for (const GameVTable *g : v->games) widest.scratch_words = std::max(widest.scratch_words, g->persist_scratch_words);
+        const size_t slot_bytes = kSnapshotRecordOff + state_record_bytes(widest);
+        const size_t source_off = align16(S * sizeof(int32_t)), load_off = source_off + align16(S * sizeof(int32_t));
+        const size_t list_off = load_off + align16(N * sizeof(int32_t)), counts_off = list_off + align16(N * sizeof(int32_t));
+        const size_t persist_off = counts_off + align16(G * sizeof(uint32_t)), slots_off = persist_off + align16(2 * G * sizeof(int32_t));
+        if (S > ((size_t)INT64_MAX - slots_off) / slot_bytes)
+            return -1;
+        const size_t bytes = slots_off + S * slot_bytes;
+        if (v->capturing())  // the allocation and the fills below would invalidate the caller's capture
+            return -1;
+        unsigned char *mem = (unsigned char *)dev_try_malloc(bytes);
+        if (!mem)
+            return -1;
+        v->owned_dev.push_back(mem);
+        v->ensure_initial_reset();
+        std::vector<int32_t> persist;
+        for (const GameVTable *g : v->games) persist.insert(persist.end(), {g->persist_scratch_first, g->persist_scratch_words});
+        memset_async(mem, 0xff, list_off, v->stream);  // save_from, source and load_from: every entry -1
+        copy_to_dev_async(mem + persist_off, persist.data(), persist.size() * sizeof(int32_t), v->stream);
+        v->sync();
+        st.slot_bytes = (int64_t)slot_bytes;
+        st.count = slots;
+        st.num_envs = v->num_envs;
+        st.games = (int32_t)G;
+        st.save_from = reinterpret_cast<int32_t *>(mem);
+        st.source = reinterpret_cast<int32_t *>(mem + source_off);
+        st.load_from = reinterpret_cast<int32_t *>(mem + load_off);
+        st.list = reinterpret_cast<int32_t *>(mem + list_off);
+        st.counts = reinterpret_cast<unsigned int *>(mem + counts_off);
+        st.persist = reinterpret_cast<const int32_t *>(mem + persist_off);
+        st.slots = mem + slots_off;  // last: pgb200_apply_snapshots reads a non-null slots pointer as the store
+        v->snap_bytes = (int64_t)bytes;
+    }
+    out->save_from = st.save_from;
+    out->load_from = st.load_from;
+    out->source = st.source;
+    out->bytes = v->snap_bytes;
+    return 0;
+}
+
+int pgb200_apply_snapshots(libenv_env *handle) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    const SnapshotStore &st = v->snaps;
+    if (!st.slots)
+        return -1;
+    const size_t G = v->games.size();
+    memset_async(st.counts, 0, G * sizeof(uint32_t), v->stream);
+#ifndef PG_HOSTSIM
+    snapshot_save_kernel<<<(st.count + 3) / 4, 128, 0, v->stream>>>(v->base, st);
+    CUDA_CHECK(cudaGetLastError());
+    snapshot_load_kernel<<<(st.num_envs + 3) / 4, 128, 0, v->stream>>>(v->base, st);
+    CUDA_CHECK(cudaGetLastError());
+#else
+    for (int s = 0; s < st.count; s++) snapshot_save(v->base, st, s);
+    for (int env = 0; env < st.num_envs; env++) snapshot_load(v->base, st, env);
+#endif
+    v->launches += 2;
+    // each game's segment of the list: its envs are at most num_envs / G
+    std::vector<size_t> first(G);
+    for (size_t g = 0; g < G; g++) first[g] = g * (size_t)(st.num_envs / st.games);
+    observe_lists(v, st.list, st.counts, first, std::vector<uint32_t>(G, (uint32_t)(st.num_envs / st.games)));
+    v->rgb_copy_enqueued = false;  // a DMA started behind the last step predates the loaded envs' frames
+    return 0;
 }
 
 int pgb200_frame_info(const char *game, int *frame_bytes, int *ctas_per_sm) {

@@ -139,6 +139,7 @@ class BaseProcgenEnv:
         self._final_outputs = None
         self._pause_mask = None
         self._rollout = None
+        self._snapshots = None
         self._num_levels, self._start_level = num_levels, start_level
         self._consumer_slot = None
         self._graph_stepped = False   # act() has run inside a CUDA graph capture
@@ -454,6 +455,67 @@ class BaseProcgenEnv:
                              "cursor": self._alias(out.cursor, (1,), "<i4")}
         return dict(self._rollout)
 
+    def snapshots(self, slots: int):
+        """{"save_from": int32 [slots], "load_from": int32 [num], "source": int32 [slots]}: CUDA tensors aliasing the
+        library's snapshot slots, a store of `slots` env states kept on the device (allocated, every entry -1, on the
+        first call). Write env indices into save_from and slot indices into load_from with torch ops on the stream you
+        step on, then call apply_snapshots(): slot s takes the state of env save_from[s], then env e takes the state of
+        slot load_from[e] and is observed as set_state observes it. Each applied entry reads -1 afterwards; an entry
+        that cannot be applied (out of range, an empty slot, a slot holding another game's state) keeps its value, so
+        `(load_from >= 0).any()` finds them. source[s] is the env whose state slot s holds, -1 while it is empty. A
+        loaded env is a byte-for-byte copy of the source env at save time: get_state() returns the blob the source
+        had, and it steps on as the source would have.
+
+        Each slot is sized for the largest live state of the handle's games (about 80 KB for coinrun), held until
+        close(); `slots` is fixed by the first call (ValueError for another value, or for slots < 1). The first call
+        cannot run inside a CUDA graph capture; the tensors may then be refilled inside one. Slots are not portable
+        across handles or processes: get_state() is the portable form."""
+        slots = int(slots)
+        if self._snapshots is not None:
+            if slots != self._snapshots["save_from"].shape[0]:
+                raise ValueError(f"snapshots(): this handle's store has {self._snapshots['save_from'].shape[0]} slots")
+            return dict(self._snapshots)
+        if slots < 1:
+            raise ValueError("snapshots(): slots must be at least 1")
+        self._refuse_in_capture("snapshots")
+        self._wait_for_replays()
+        torch = self._torch
+        out = L.Snapshots()
+        with torch.cuda.device(self.device_index):
+            if self._lib.pgb200_get_snapshots(self._h, slots, C.byref(out)) != 0:
+                raise RuntimeError(f"pgb200_get_snapshots failed: {slots} slots could not be allocated")
+            self._snapshots = {"save_from": self._alias(out.save_from, (slots,), "<i4"),
+                               "load_from": self._alias(out.load_from, (self.num,), "<i4"),
+                               "source": self._alias(out.source, (slots,), "<i4")}
+        return dict(self._snapshots)
+
+    def apply_snapshots(self) -> None:
+        """Apply the saves and loads written into snapshots()' arrays: every save first, then every load, then the
+        loaded envs' observations, on the current torch stream (as act(), it rebinds the handle to it). It never waits
+        for the host, so it may run inside torch.cuda.graph; a replay applies the arrays as they are then. Envs not
+        loaded, the rollout, final outputs, the pause mask, next_level_seeds(), the bank and lookahead are untouched."""
+        if self._snapshots is None:
+            raise RuntimeError("apply_snapshots(): call snapshots(slots) first")
+        torch = self._torch
+        if self._host_buffers:
+            self._refuse_in_capture("apply_snapshots")
+            # the library works on its own stream here: the caller's torch writes must be complete first, and its
+            # reads of the arrays must see the apply
+            torch.cuda.current_stream(self._snapshots["save_from"].device).synchronize()
+            rc = self._lib.pgb200_apply_snapshots(self._h)
+            self._lib.pgb200_sync(self._h)
+        else:
+            with torch.cuda.device(self._dev):
+                cur = torch.cuda.current_stream(self._dev).cuda_stream
+                if cur != self._stream_handle:
+                    self._lib.pgb200_set_stream(self._h, C.c_void_p(cur))
+                    self._stream_handle = cur
+                if self._capturing():
+                    self._graph_stepped = True
+                rc = self._lib.pgb200_apply_snapshots(self._h)
+        if rc != 0:
+            raise RuntimeError("pgb200_apply_snapshots failed")
+
     def build_level_bank(self, seeds=None, capacity: int = 0) -> None:
         """Bank the levels of `seeds` (default: range(start_level, start_level + num_levels)) for every game of the
         handle: a reset inside a step onto a banked seed copies the level generated here instead of generating it
@@ -761,6 +823,7 @@ class BaseProcgenEnv:
             self._final_outputs = None
             self._pause_mask = None
             self._rollout = None
+            self._snapshots = None
             self._lib.libenv_close(self._h)
             self._h = None
 

@@ -49,6 +49,10 @@ class Rollout(C.Structure):
     _fields_ = [("rgb", C.c_void_p), ("rew", C.c_void_p), ("first", C.c_void_p), ("cursor", C.c_void_p)]
 
 
+class Snapshots(C.Structure):
+    _fields_ = [("save_from", C.c_void_p), ("load_from", C.c_void_p), ("source", C.c_void_p), ("bytes", C.c_int64)]
+
+
 class DeviceBuffers(C.Structure):
     _fields_ = [("rgb", C.c_void_p), ("rew", C.c_void_p), ("first", C.c_void_p), ("prev_level_seed", C.c_void_p),
                 ("prev_level_complete", C.c_void_p), ("level_seed", C.c_void_p), ("action", C.c_void_p),
@@ -63,7 +67,8 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_set_consumer_output", "pgb200_consumer_slot", "pgb200_debug_phase_offset", "pgb200_get_next_level_seeds",
            "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
            "pgb200_build_level_bank", "pgb200_level_bank_info", "pgb200_enable_level_lookahead",
-           "pgb200_level_lookahead_info", "pgb200_get_rollout", "pgb200_get_states", "pgb200_set_states"]
+           "pgb200_level_lookahead_info", "pgb200_get_rollout", "pgb200_get_states", "pgb200_set_states",
+           "pgb200_get_snapshots", "pgb200_apply_snapshots"]
 
 _lib = None
 
@@ -128,6 +133,10 @@ def bind(lib):
     lib.pgb200_get_states.restype = C.c_int
     lib.pgb200_set_states.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_char_p, C.POINTER(C.c_int64)]
     lib.pgb200_set_states.restype = C.c_int
+    lib.pgb200_get_snapshots.argtypes = [C.c_void_p, C.c_int, C.POINTER(Snapshots)]
+    lib.pgb200_get_snapshots.restype = C.c_int
+    lib.pgb200_apply_snapshots.argtypes = [C.c_void_p]
+    lib.pgb200_apply_snapshots.restype = C.c_int
     lib.pgb200_set_launch_shape.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.pgb200_set_launch_shape.restype = None
     lib.pgb200_kernel_timing_begin.argtypes = [C.c_void_p, C.c_int]
