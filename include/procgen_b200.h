@@ -229,6 +229,25 @@ LIBENV_API int pgb200_get_final_outputs(libenv_env *handle, struct pgb200_final_
  * then reads its contents at every replay. A handle without the mask runs the kernels it ran before. */
 LIBENV_API int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out);
 
+/* Action repeat (frame skip): `*out` = this handle's int32 array repeat[num_envs] (device memory; host memory in
+ * the CPU debug build), allocated with every entry 1 by the first call, which also performs the initial reset if
+ * it has not happened yet. Returns 0. The pointer stays valid until libenv_close. A step reads the array and
+ * never changes it. In every step, an env e with repeat[e] = r:
+ *   - plays max(r, 1) game steps (Game::step) with its action, and stops after the first whose level ends (game
+ *     end, time limit, action -1, or a completed level with use_sequential_levels). Action -1 thus plays one, and
+ *     the time limit bounds the game steps of any r;
+ *   - reports rew[e] = the float sum of those game steps' rewards, in order; first[e], the three info slots and,
+ *     with final outputs, level_end[e] are the last game step's, and rgb[e] is the frame of the final state. The
+ *     final rgb[e] of final outputs is the frame of the state the level ended in;
+ *   - takes its next_level_seed entry at the one reset the step can contain, as without action repeat.
+ * A paused env (pgb200_get_pause_mask) plays no game step, whatever its entry. The rollout and the consumer ring
+ * move on once per step. get_state / set_state, snapshots, the level bank and level lookahead neither read nor
+ * write the array. An all-ones array gives the outputs and states of a handle that never called this, which runs
+ * the kernels it ran before. Ordering and CUDA graphs as for the pause mask: the first call is refused (-1) while
+ * the handle's stream captures, and a captured step reads the array only if it existed at capture, then reads its
+ * contents at every replay. */
+LIBENV_API int pgb200_get_action_repeat(libenv_env *handle, int32_t **out);
+
 /* Level bank: levels generated once and copied in at reset. A generated level is a pure function of the game, the
  * options and the seed, so a handle that keeps resetting onto the same few hundred seeds (num_levels = 200 or
  * 500, a held-out seed list, a level-replay buffer) can keep them instead of generating them again.
@@ -391,13 +410,15 @@ LIBENV_API void pgb200_set_stream(libenv_env *handle, void *stream);
  * replay is the step issued at capture: same outputs as an eager call on the same inputs.
  * A captured step keeps what the host decided at capture: the launch shape (pgb200_set_launch_shape), the
  * level choice (the next_level_seed array is read only if pgb200_get_next_level_seeds had been called
- * before the capture; likewise the pause mask and pgb200_get_pause_mask), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
+ * before the capture; likewise the pause mask and pgb200_get_pause_mask, and the action repeat counts and
+ * pgb200_get_action_repeat), the consumer output's buffer, dtype and k, and the handle's device buffers. Changing
  * any of these afterwards leaves the graph as it was; capture again. Replays of one handle's graphs must be
  * ordered with each other and with its eager work (one stream, or events). pgb200_kernel_launches counts
  * launches issued, a captured step once, not its replays. pgb200_apply_snapshots may be captured the same way.
  * Refused while the handle's stream is capturing (they wait for the device or allocate; -1, UINT32_MAX for
  * pgb200_get_errors, or a fatal message where the call returns nothing): the first
- * pgb200_get_next_level_seeds, pgb200_get_final_outputs and pgb200_get_pause_mask, pgb200_build_level_bank,
+ * pgb200_get_next_level_seeds, pgb200_get_final_outputs, pgb200_get_pause_mask and pgb200_get_action_repeat,
+ * pgb200_build_level_bank,
  * the first pgb200_enable_level_lookahead, pgb200_level_lookahead_info, the first pgb200_get_rollout, the first pgb200_get_snapshots, pgb200_get_device_buffers
  * before the initial reset, pgb200_set_consumer_output,
  * pgb200_set_rgb_mirror, get_state, set_state, pgb200_get_errors, pgb200_debug_cycles, pgb200_debug_read_env,

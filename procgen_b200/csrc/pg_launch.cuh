@@ -83,7 +83,9 @@ constexpr int kRenderThreads = 128;
 // FINAL: phase A of a step with final outputs; an env whose level ends is appended to p.reset_list.
 // PAUSE: the handle has a pause mask. A paused env's warp reads its entry, writes its outputs and takes the next
 // ticket without touching the env's state; it never enters phase B's list.
-template <class G, bool INIT, bool LEVEL_CHOICE = false, bool FINAL = false, bool PAUSE = false>
+// REPEAT: the handle has action repeat. A warp plays up to repeat[env] game steps of its env; the tickets spread the
+// uneven work as they spread level generation.
+template <class G, bool INIT, bool LEVEL_CHOICE = false, bool FINAL = false, bool PAUSE = false, bool REPEAT = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -96,7 +98,7 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
             break;
         const int env = p.env_first + (int)t * p.env_step;
         const long long t0 = p.dbg_cycles ? clock64() : 0;
-        env_logic<G, Frame, INIT, LEVEL_CHOICE, FINAL, PAUSE>(p, env);
+        env_logic<G, Frame, INIT, LEVEL_CHOICE, FINAL, PAUSE, REPEAT>(p, env);
         __syncwarp();
         if (p.dbg_cycles && lane == 0)
             p.dbg_cycles[env] = (uint32_t)(clock64() - t0);
@@ -108,7 +110,8 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) logic_kern
 // BANK: the handle has a level bank; the only kernel a banked step adds to those of an unbanked one.
 // LOOK: the handle has level lookahead: resets copy from the env's lookahead slot where it holds their level, and list
 // the envs whose next level lookahead_kernel generates.
-template <class G, bool BANK = false, bool LOOK = false>
+// REPEAT: the handle has action repeat; a reset's reward joins the sum phase A left in rew.
+template <class G, bool BANK = false, bool LOOK = false, bool REPEAT = false>
 __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_kernel(KParams p, unsigned int *ticket) {
     using Frame = typename FrameFor<G>::type;
     const unsigned lane = threadIdx.x & 31u;
@@ -123,7 +126,7 @@ __global__ void __launch_bounds__(kLogicThreads, PG_LOGIC_MIN_BLOCKS) finish_ker
         const int env = p.reset_list[t];
         // a banked step's reset runs here: its cycles join phase A's in the profiling aid
         const long long t0 = ((BANK || LOOK) && p.dbg_cycles) ? clock64() : 0;
-        env_finish_logic<G, Frame, BANK, LOOK>(p, env);
+        env_finish_logic<G, Frame, BANK, LOOK, REPEAT>(p, env);
         __syncwarp();
         if ((BANK || LOOK) && p.dbg_cycles && lane == 0)
             p.dbg_cycles[env] += (uint32_t)(clock64() - t0);
@@ -521,6 +524,7 @@ struct StepShape {
     bool bank = false;           // level bank
     bool look = false;           // level lookahead: its kernel follows phase B
     bool roll = false;           // rollout: the render kernel's ROLL instantiation, and a cursor advance per step
+    bool repeat = false;         // action repeat: the logic and finish kernels' REPEAT instantiations
     // A step in two phases: the logic kernel (phase A) lists the envs whose level ends, and the finish kernel (phase B)
     // resets them. Its logic kernel is one that steps always run (its stack frame and registers stay those of the
     // step, which must fit the push_obj / sub_step recursion).
@@ -585,14 +589,14 @@ static inline int logic_grid(const KParams &p, const LaunchCtx &lc) {
 // logic: clears the words of the launch's ticket slot the step uses, then runs the logic kernel over the launch's envs.
 // A two-phase step stays on lc.stream: a priority-split logic stream would let the next launch that shares this ticket
 // slot clear it under phase B. A one-phase step's logic kernel may go to that stream (PGB200_PRIORITY_SPLIT).
-template <class G, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE>
+template <class G, bool INIT, bool LEVEL_CHOICE, bool FINAL, bool PAUSE, bool REPEAT>
 void logic_kernels(const KParams &p, const LaunchCtx &lc, size_t ticket_bytes) {
 #ifndef PG_HOSTSIM
     const cudaStream_t ls = !FINAL && lc.logic_stream ? lc.logic_stream : lc.stream;
     CUDA_CHECK(cudaMemsetAsync(lc.ticket, 0, ticket_bytes, ls));
     if (lc.tev)
         CUDA_CHECK(cudaEventRecord(lc.tev[0], ls));
-    logic_kernel<G, INIT, LEVEL_CHOICE, FINAL, PAUSE><<<logic_grid(p, lc), kLogicThreads, 0, ls>>>(p, &lc.ticket->logic);
+    logic_kernel<G, INIT, LEVEL_CHOICE, FINAL, PAUSE, REPEAT><<<logic_grid(p, lc), kLogicThreads, 0, ls>>>(p, &lc.ticket->logic);
     CUDA_CHECK(cudaGetLastError());
     if (ls != lc.stream) {
         CUDA_CHECK(cudaEventRecord(lc.link, ls));
@@ -601,39 +605,46 @@ void logic_kernels(const KParams &p, const LaunchCtx &lc, size_t ticket_bytes) {
 #else
     using Frame = typename FrameFor<G>::type;
     memset(lc.ticket, 0, ticket_bytes);
-    for (int i = 0; i < p.env_count; i++) env_logic<G, Frame, INIT, LEVEL_CHOICE, FINAL, PAUSE>(p, p.env_first + i * p.env_step);
+    for (int i = 0; i < p.env_count; i++) env_logic<G, Frame, INIT, LEVEL_CHOICE, FINAL, PAUSE, REPEAT>(p, p.env_first + i * p.env_step);
 #endif
     (*lc.launch_counter) += 1;
 }
 
-// INIT, or a step: FINAL (phase A) when it has two phases, LEVEL_CHOICE only when it has one, PAUSE with a pause mask
+// INIT, or a step: FINAL (phase A) when it has two phases, LEVEL_CHOICE only when it has one, PAUSE with a pause mask,
+// REPEAT with action repeat
 template <class G>
 void logic_phase(const KParams &p, const LaunchCtx &lc, const StepShape &s) {
     if (s.init)
-        return logic_kernels<G, true, false, false, false>(p, lc, s.ticket_bytes());
-    with_flag(s.pause, [&](auto pause) {
-        with_flag(s.two_phase(), [&](auto final) {
-            if constexpr (final)
-                logic_kernels<G, false, false, true, pause>(p, lc, s.ticket_bytes());
-            else
-                with_flag(s.level_choice, [&](auto choice) { logic_kernels<G, false, choice, false, pause>(p, lc, s.ticket_bytes()); });
+        return logic_kernels<G, true, false, false, false, false>(p, lc, s.ticket_bytes());
+    with_flag(s.repeat, [&](auto repeat) {
+        with_flag(s.pause, [&](auto pause) {
+            with_flag(s.two_phase(), [&](auto final) {
+                if constexpr (final)
+                    logic_kernels<G, false, false, true, pause, repeat>(p, lc, s.ticket_bytes());
+                else
+                    with_flag(s.level_choice,
+                              [&](auto choice) { logic_kernels<G, false, choice, false, pause, repeat>(p, lc, s.ticket_bytes()); });
+            });
         });
     });
 }
 
 // finish: phase B's resets, the finish kernel over the envs phase A listed. BANK: they copy their levels from the
 // bank where it holds them. LOOK: or from their lookahead slots, and list the envs whose next level is to be generated.
+// REPEAT: their rew adds the reset's reward to phase A's sum.
 template <class G>
 void finish_phase(const KParams &p, const LaunchCtx &lc, const StepShape &s) {
     with_flag(s.bank, [&](auto bank) {
         with_flag(s.look, [&](auto look) {
+            with_flag(s.repeat, [&](auto repeat) {
 #ifndef PG_HOSTSIM
-            finish_kernel<G, bank, look><<<logic_grid(p, lc), kLogicThreads, 0, lc.stream>>>(p, &lc.ticket->finish);
-            CUDA_CHECK(cudaGetLastError());
+                finish_kernel<G, bank, look, repeat><<<logic_grid(p, lc), kLogicThreads, 0, lc.stream>>>(p, &lc.ticket->finish);
+                CUDA_CHECK(cudaGetLastError());
 #else
-            using Frame = typename FrameFor<G>::type;
-            for (unsigned int j = 0; j < *p.reset_count; j++) env_finish_logic<G, Frame, bank, look>(p, p.reset_list[j]);
+                using Frame = typename FrameFor<G>::type;
+                for (unsigned int j = 0; j < *p.reset_count; j++) env_finish_logic<G, Frame, bank, look, repeat>(p, p.reset_list[j]);
 #endif
+            });
         });
     });
     (*lc.launch_counter) += 1;

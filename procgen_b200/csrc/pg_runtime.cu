@@ -338,8 +338,10 @@ struct VecEnv {
     // pause (the caller's mask, d_pause) and paused (what the logic kernel recorded of it for the step's later
     // kernels) by pgb200_get_pause_mask; bank_level_end by the first pgb200_build_level_bank. reset_list, the
     // pending-reset list of a two-phase step, by whichever of final outputs and the bank comes first. The rollout
-    // (base.roll) by the first pgb200_get_rollout.
+    // (base.roll) by the first pgb200_get_rollout. The caller's repeat counts (d_repeat, base.repeat) by the first
+    // pgb200_get_action_repeat.
     uint8_t *d_pause = nullptr;
+    int32_t *d_repeat = nullptr;
     // allocated by the first pgb200_build_level_bank: bank_capacity slots per game of the list, sized by the game
     // (banks[g], one allocation at base.bank.slots), the sorted seed list they share and its length on the device
     std::vector<LevelBank> banks;
@@ -506,6 +508,7 @@ struct VecEnv {
         s.bank = base.bank.slots != nullptr;
         s.look = base.look.slot.slots != nullptr;
         s.roll = base.roll.rgb != nullptr;
+        s.repeat = base.repeat != nullptr;
         return s;
     }
 
@@ -1246,6 +1249,22 @@ int pgb200_get_pause_mask(libenv_env *handle, uint8_t **out) {
     v->opt_in_array(v->d_pause, 1, 0);
     v->base.pause = v->d_pause;  // last: VecEnv::step_shape reads a non-null pause as the mask on
     *out = v->d_pause;
+    return 0;
+}
+
+int pgb200_get_action_repeat(libenv_env *handle, int32_t **out) {
+    VecEnv *v = (VecEnv *)handle;
+    v->set_device();
+    if (!v->begin_opt_in(v->d_repeat != nullptr))
+        return -1;
+    if (!v->d_repeat) {
+        v->opt_in_array(v->d_repeat, 1, 0);
+        const std::vector<int32_t> ones((size_t)std::max(v->num_envs, 1), 1);
+        copy_to_dev_async(v->d_repeat, ones.data(), ones.size() * sizeof(int32_t), v->stream);
+        v->sync();
+    }
+    v->base.repeat = v->d_repeat;  // last: VecEnv::step_shape reads a non-null repeat as action repeat on
+    *out = v->d_repeat;
     return 0;
 }
 

@@ -138,6 +138,7 @@ class BaseProcgenEnv:
         self._next_level_seeds = None
         self._final_outputs = None
         self._pause_mask = None
+        self._action_repeat = None
         self._rollout = None
         self._snapshots = None
         self._num_levels, self._start_level = num_levels, start_level
@@ -276,9 +277,9 @@ class BaseProcgenEnv:
         Inside ``torch.cuda.graph`` (or any capture on the current stream) act() takes a CUDA tensor only and
         the step becomes part of the graph: the handle is rebound to the capture stream without a host wait,
         and every replay steps the envs again with whatever the action tensor then holds. Set up before the
-        capture what the step should use (next_level_seeds(), pause_mask(), enable_consumer_output(), rollout(),
-        set_launch_shape()): a graph keeps the launch shape, the level choice, the pause mask, the consumer output and
-        the rollout it was captured with."""
+        capture what the step should use (next_level_seeds(), pause_mask(), action_repeat(), enable_consumer_output(),
+        rollout(), set_launch_shape()): a graph keeps the launch shape, the level choice, the pause mask, the action
+        repeat, the consumer output and the rollout it was captured with."""
         if self._capturing():
             if self._host_buffers:
                 raise RuntimeError("procgen_b200: act() cannot be captured in a CUDA graph with host_buffers=True; "
@@ -294,10 +295,10 @@ class BaseProcgenEnv:
             self._graph_stepped = True
         if self._host_buffers:
             self._ac[:] = np.asarray(ac).astype(np.int32)
-            for arr in (self._next_level_seeds, self._pause_mask):
+            for arr in (self._next_level_seeds, self._pause_mask, self._action_repeat):
                 if arr is not None:
-                    # libenv_act reads the level choices and the pause mask on the library's own stream: the
-                    # caller's torch writes must be complete first
+                    # libenv_act reads the level choices, the pause mask and the repeat counts on the library's
+                    # own stream: the caller's torch writes must be complete first
                     self._torch.cuda.current_stream(arr.device).synchronize()
                     break
             self._lib.libenv_act(self._h)
@@ -420,6 +421,33 @@ class BaseProcgenEnv:
                     raise RuntimeError("pgb200_get_pause_mask failed")
                 self._pause_mask = self._alias(ptr, (self.num,), "|u1")
         return self._pause_mask
+
+    def action_repeat(self):
+        """int32 CUDA tensor [num] aliasing the library's per-env action repeat counts (allocated, all 1, on the first
+        call). In every step, env e with entry r plays max(r, 1) game steps with its action and stops after the first
+        whose level ends (game end, time limit, action -1, or a completed level with use_sequential_levels), so
+        action -1 plays one. rew[e] is the float32 sum of those game steps' rewards, in order; first[e], the info
+        slots and final_outputs()["level_end"][e] are the last one's, and rgb[e] is the frame of the final state
+        (final_outputs()["rgb"][e] that of the state the level ended in). The env takes its next_level_seeds() entry
+        at the one reset a step can contain. A paused env (pause_mask()) plays no game step. The rollout and the
+        consumer output move on once per act(). A step does not change the array; get_state / set_state, snapshots,
+        the level bank and lookahead neither read nor change it. An all-ones array steps exactly as a handle that
+        never called this.
+
+        Write it with torch ops on the stream you step on (device-resident mode); with host_buffers=True, act()
+        waits for the current torch stream before it starts the step.
+
+        A CUDA graph reads the array only if it was requested before the capture: call this once first. Inside the
+        capture the tensor may then be refilled with torch ops like any other input of the graph."""
+        if self._action_repeat is None:
+            self._refuse_in_capture("action_repeat")
+            torch = self._torch
+            ptr = C.POINTER(C.c_int32)()
+            with torch.cuda.device(self.device_index):
+                if self._lib.pgb200_get_action_repeat(self._h, C.byref(ptr)) != 0:
+                    raise RuntimeError("pgb200_get_action_repeat failed")
+                self._action_repeat = self._alias(ptr, (self.num,), "<i4")
+        return self._action_repeat
 
     def rollout(self, slots: int):
         """{"rgb": uint8 [slots, num, 64, 64, 3], "rew": float32 [slots, num], "first": uint8 [slots, num], "cursor": int32
@@ -822,6 +850,7 @@ class BaseProcgenEnv:
             self._next_level_seeds = None
             self._final_outputs = None
             self._pause_mask = None
+            self._action_repeat = None
             self._rollout = None
             self._snapshots = None
             self._lib.libenv_close(self._h)

@@ -68,7 +68,7 @@ EXPORTS = ["libenv_version", "libenv_make", "libenv_get_tensortypes", "libenv_se
            "pgb200_get_consumer_slot_device", "pgb200_get_final_outputs", "pgb200_get_pause_mask",
            "pgb200_build_level_bank", "pgb200_level_bank_info", "pgb200_enable_level_lookahead",
            "pgb200_level_lookahead_info", "pgb200_get_rollout", "pgb200_get_states", "pgb200_set_states",
-           "pgb200_get_snapshots", "pgb200_apply_snapshots"]
+           "pgb200_get_snapshots", "pgb200_apply_snapshots", "pgb200_get_action_repeat"]
 
 _lib = None
 
@@ -92,6 +92,8 @@ def bind(lib):
     lib.pgb200_get_final_outputs.restype = C.c_int
     lib.pgb200_get_pause_mask.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8))]
     lib.pgb200_get_pause_mask.restype = C.c_int
+    lib.pgb200_get_action_repeat.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
+    lib.pgb200_get_action_repeat.restype = C.c_int
     lib.pgb200_build_level_bank.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int]
     lib.pgb200_build_level_bank.restype = C.c_int
     lib.pgb200_level_bank_info.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int64)]
